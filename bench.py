@@ -1,15 +1,18 @@
-"""bench.py — BigGAN-Deep 256x256 G+D step throughput (BASELINE.json config 4) on N B200s, one JSON line on rank 0.
+"""bench.py — BigGAN-Deep 256x256 G+D step throughput (BASELINE.json config 4) on N H100s, one JSON line on rank 0.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--config yaml]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--config yaml] [--dump-outputs DIR]
 
 step     = WORKER.train_discriminator (d_updates_per_step = 2 discriminator updates) + WORKER.train_generator
            (one generator update + EMA), i.e. one iteration of the reference loop (src/loader.py:392-398).
 metric   = images/s = global batch x acml_steps / step time, whole job over all ranks (strong scaling: the global
-           batch is fixed at 256, each rank takes 256/N).
+           batch is fixed at 256, each rank takes 256/N; a rank whose share does not fit in its GPU runs it as accumulated
+           micro-batches, see PER_RANK_BATCH_LIMIT).
 value    = synthetic real images already resident in HBM.
 e2e      = the same step driven from pinned HOST buffers: the basket's H2D copy and a D2H read of both losses are inside
            the timed region.
 --impl reference : the CPU path (oracle port of the reference step) on the host cores, bounded sample, rank 0 only.
+--dump-outputs DIR : after the timed steps, what the last timed step returned and updated (both losses, a fixed seeded
+           sample of the generator / discriminator / EMA-generator state) as DIR/<name>.npy, for comparing two builds.
 """
 import argparse
 import json
@@ -42,6 +45,10 @@ METRIC_NAME = {"BigGAN-Deep-256res": "BigGAN-Deep 256x256 G+D step images/sec",
 # (yaml, the world sizes it is run at)
 ALSO = [("SNGAN-CIFAR10-b256", (1,)), ("BigGAN-CIFAR10-b512", (1, 2, 4)), ("WGAN-GP-128res", (1, 2))]
 G_FWD_GF, D_FWD_GF = 58.80, 60.50
+# Largest per-rank batch whose saved activations fit in an 80 GB H100 (BigGAN-Deep 256x256 at 256 images needs ~100 GB in
+# the G phase).  A larger share of the global batch is split into equal micro-batches accumulated over acml_steps: the same
+# images and optimiser steps, with batch-norm statistics per micro-batch.
+PER_RANK_BATCH_LIMIT = {"BigGAN-Deep-256res": 128}
 
 
 def parse():
@@ -61,6 +68,8 @@ def parse():
     ap.add_argument("--fid-num", type=int, default=50000)
     ap.add_argument("--cpu-batch", type=int, default=4, help="images per CPU-baseline step (4 -> ~15 s of CPU work on 32 threads)")
     ap.add_argument("--cpu-threads", type=int, default=0, help="0 = min(32, host cores): more threads only add contention for these layer sizes")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     return ap.parse_args()
 
 
@@ -140,6 +149,12 @@ def build_worker(args, rank, world, device, config_path=None):
     global_batch = cfgs.OPTIMIZATION.batch_size
     assert global_batch % world == 0
     cfgs.OPTIMIZATION.batch_size = global_batch // world           # per-rank batch, as src/loader.py:162
+    limit = PER_RANK_BATCH_LIMIT.get(os.path.splitext(os.path.basename(config_path or args.config))[0])
+    if limit and cfgs.OPTIMIZATION.batch_size > limit:
+        split = -(-cfgs.OPTIMIZATION.batch_size // limit)
+        assert cfgs.OPTIMIZATION.batch_size % split == 0
+        cfgs.OPTIMIZATION.batch_size //= split
+        cfgs.OPTIMIZATION.acml_steps *= split
     cfgs.RUN.cuda_graphs = args.graphs == "on" or (args.graphs == "auto" and cfgs.OPTIMIZATION.batch_size <= 64)
     cfgs.OPTIMIZATION.world_size = world
     cfgs.RUN.distributed_data_parallel = world > 1
@@ -157,14 +172,42 @@ def build_worker(args, rank, world, device, config_path=None):
     return cfgs, worker, global_batch
 
 
+def images_per_step(cfgs, world):
+    """Images consumed by one optimiser step over all ranks: micro-batch x ranks x accumulation steps."""
+    return cfgs.OPTIMIZATION.batch_size * world * cfgs.OPTIMIZATION.acml_steps
+
+
 def run_steps(worker, n, read_losses):
+    """Runs n steps; returns the last step's (d_loss, g_loss): floats when read_losses (a D2H read per step), else tensors."""
     out = None
     for s in range(n):
         _, d_loss = worker.train_discriminator(s)
         g_loss = worker.train_generator(s)
+        out = (d_loss, g_loss)
         if read_losses:
             out = (float(d_loss.detach()), float(g_loss.detach()))      # D2H read of the step's results
     return out
+
+
+DUMP_STATE_SAMPLE = 4 << 20          # elements per network state sampled by --dump-outputs (3 x 16 MB float32)
+
+
+def dump_outputs(dump_dir, worker, losses):
+    """What the last timed step handed back and left behind: both losses (float64) and, per network (G, D, EMA G), a fixed
+    seeded sample of its floating-point state (parameters + buffers, state_dict order) in float32."""
+    os.makedirs(dump_dir, exist_ok=True)
+    d_loss, g_loss = losses
+    np.save(os.path.join(dump_dir, "d_loss.npy"), np.array([float(d_loss.detach())], dtype=np.float64))
+    np.save(os.path.join(dump_dir, "g_loss.npy"), np.array([float(g_loss.detach())], dtype=np.float64))
+    for name, net in (("G_state", worker.Gen), ("D_state", worker.Dis), ("G_ema_state", worker.Gen_ema)):
+        if net is None:
+            continue
+        flat = torch.cat([t.detach().reshape(-1).float() for t in net.state_dict().values() if t.is_floating_point()])
+        if flat.numel() > DUMP_STATE_SAMPLE:
+            idx = torch.randint(flat.numel(), (DUMP_STATE_SAMPLE,), generator=torch.Generator().manual_seed(1234)).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(dump_dir, name + ".npy"), flat.cpu().numpy().astype(np.float32))
+        del flat
 
 
 def timed(worker, steps, world, read_losses):
@@ -201,7 +244,7 @@ def fid_eval_seconds(worker, cfgs, device, num_eval, batch, world=1):
             if n > 0:
                 yield torch.randint(0, 256, (n, 3, S, S), generator=gen, device=device).float()
     # load cuSOLVER (the Frechet distance's two symmetric eigendecompositions) before anything is timed: on a fresh box the first
-    # call pages the library in from disk, measured at 0.2 s to 30 s for the same code (profiles/r02_fid_n2_eval_phases.txt)
+    # call pages the library in from disk, which can take seconds
     _a = torch.randn(2048, 2048, dtype=torch.float64, device=device)
     _a = _a @ _a.t()
     torch.linalg.eigh(_a)
@@ -330,7 +373,7 @@ def config_dict(workload, cfgs_or_none, global_batch, world, graphs, S, d_update
     per_rank = global_batch // world
     return {"workload": workload, "global_batch": global_batch, "per_gpu_batch": per_rank, "img_size": S,
             "d_updates_per_step": d_updates, "acml_steps": acml, "parallelism": "dp%d" % world, "cuda_graphs": bool(graphs),
-            "l2": "per-step working set (tens of GB of activations) >> 126 MB L2; no explicit flush needed"}
+            "l2": "per-step working set (tens of GB of activations) >> 50 MB L2; no explicit flush needed"}
 
 
 def graphs_wanted(args, per_rank):
@@ -366,8 +409,9 @@ def reference_arm(args, workload):
             "e2e": {"value": v, "unit": "img/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}, "gpu_launches": 0}
 
 
-def measure(args, rank, world, device, config_path, steps, warmup, want_e2e, want_profile):
-    """Warm-up + timed steps of one workload (device-resident baskets), optional per-kernel accounting step and e2e leg."""
+def measure(args, rank, world, device, config_path, steps, warmup, want_e2e, want_profile, dump_dir=None):
+    """Warm-up + timed steps of one workload (device-resident baskets), optional output dump, per-kernel accounting step and
+    e2e leg."""
     from sgb200 import _lib
     cfgs, worker, global_batch = build_worker(args, rank, world, device, config_path)
     opt = cfgs.OPTIMIZATION
@@ -381,11 +425,14 @@ def measure(args, rank, world, device, config_path, steps, warmup, want_e2e, wan
     if rank == 0:
         sampler.start()
     launches0 = _lib.LAUNCHES[0]
-    ms_step, _ = timed(worker, steps, world, False)
+    ms_step, last = timed(worker, steps, world, False)
     launches = (_lib.LAUNCHES[0] - launches0)
     sampler.stop_flag = True
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, worker, last)
     res = {"cfgs": cfgs, "worker": worker, "global_batch": global_batch, "per_rank": per_rank, "S": S, "ms_step": ms_step,
-           "value": global_batch * opt.acml_steps / (ms_step * 1e-3), "launches": launches, "clocks": sampler.summary() if rank == 0 else None,
+           "images_per_step": images_per_step(cfgs, world),
+           "value": images_per_step(cfgs, world) / (ms_step * 1e-3), "launches": launches, "clocks": sampler.summary() if rank == 0 else None,
            "graphs_captured": {n: bool(getattr(getattr(worker, n, None), "graph", None) is not None) for n in ("_d_graph", "_g_graph")},
            "prof": None, "prof_by_tag": None, "e2e": None}
     if want_profile:
@@ -394,10 +441,8 @@ def measure(args, rank, world, device, config_path, steps, warmup, want_e2e, wan
             _lib.PROFILE["enabled"] = True
             graphs_on, cfgs.RUN.cuda_graphs = cfgs.RUN.cuda_graphs, False      # the accounting step runs eagerly (events per call)
             torch.cuda.synchronize()
-            w0 = time.perf_counter()
             run_steps(worker, 1, False)
             torch.cuda.synchronize()
-            prof_wall_ms = (time.perf_counter() - w0) * 1e3
             _lib.PROFILE["enabled"] = False
             cfgs.RUN.cuda_graphs = graphs_on
             agg, by_tag = {}, {}
@@ -411,12 +456,6 @@ def measure(args, rank, world, device, config_path, steps, warmup, want_e2e, wan
                                "flop": v[1], "gbytes": v[3] * 1e-9, "gb_per_s": (v[3] / (v[0] * 1e-3) * 1e-9) if v[0] > 0 and v[3] > 0 else None}
                            for k, v in agg.items()}
             res["prof_by_tag"] = by_tag
-            if rank == 0:
-                os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-                with open(os.path.join(ROOT, "gpurun_out", "kernel_breakdown_n%d_b%d.json" % (world, global_batch)), "w") as fh:
-                    json.dump({"wall_ms_of_profiled_step": prof_wall_ms, "sum_ms": sum(v[0] for v in agg.values()), "by_kind": res["prof"],
-                               "by_tag": [{"tag": k, "ms": v[0], "n": v[2], "flop": v[1], "bytes": v[3]} for k, v in
-                                          sorted(by_tag.items(), key=lambda kv: -kv[1][0])]}, fh, indent=1)
         except Exception as ex:  # accounting must never take the bench line down
             _lib.PROFILE["enabled"] = False
             res["prof"] = {"error": repr(ex)}
@@ -432,7 +471,7 @@ def measure(args, rank, world, device, config_path, steps, warmup, want_e2e, wan
         worker.train_dataloader, worker.train_iter = host_loader, iter(host_loader)
         run_steps(worker, 1, True)
         ms_e2e, _ = timed(worker, steps, world, True)
-        res["e2e"] = {"value": global_batch * opt.acml_steps / (ms_e2e * 1e-3), "unit": "img/s",
+        res["e2e"] = {"value": images_per_step(cfgs, world) / (ms_e2e * 1e-3), "unit": "img/s",
                       "h2d_bytes_per_step": world * host_loader.h2d_bytes, "d2h_bytes_per_step": 8 * world, "ms_per_step": ms_e2e,
                       "input": "uint8 NHWC baskets from pinned host memory (%d B/step/rank), device-side flip + normalise" % host_loader.h2d_bytes}
         worker.train_dataloader = worker.train_iter = None
@@ -484,7 +523,7 @@ def main():
         except Exception as ex:  # noqa: BLE001
             mr_check = {"ok": False, "error": repr(ex)}
 
-    res = measure(args, rank, world, device, None, args.steps, args.warmup, not args.no_e2e, True)
+    res = measure(args, rank, world, device, None, args.steps, args.warmup, not args.no_e2e, True, args.dump_outputs)
     cfgs, worker, global_batch, per_rank, S = res["cfgs"], res["worker"], res["global_batch"], res["per_rank"], res["S"]
     opt = cfgs.OPTIMIZATION
     ms_step, value, prof = res["ms_step"], res["value"], res["prof"]
@@ -506,7 +545,7 @@ def main():
             try:
                 r = measure(args, rank, world, device, os.path.join(PKG, "configs", name + ".yaml"), max(3, min(args.steps, 10)), 3,
                             True, False)
-                gf = STEP_GFLOP_PER_IMAGE.get(name, 0.0) * 1e9 * r["global_batch"]
+                gf = STEP_GFLOP_PER_IMAGE.get(name, 0.0) * 1e9 * r["images_per_step"]
                 also[name] = {"metric": METRIC_NAME[name], "value": r["value"], "unit": "img/s", "ms_per_step": r["ms_step"],
                               "global_batch": r["global_batch"], "img_size": r["S"], "d_updates_per_step": r["cfgs"].OPTIMIZATION.d_updates_per_step,
                               "e2e": r["e2e"], "gpu_launches": r["launches"], "cuda_graphs_captured": r["graphs_captured"],
@@ -524,39 +563,31 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained" if "bf16_tflops_sustained" in peaks else "fallback 1.4 PFLOP/s sustained"
-    step_flop = STEP_GFLOP_PER_IMAGE.get(workload, 0.0) * 1e9 * global_batch
-    # roofline.traffic: DRAM bytes per launch of the dominant kernel from this round's committed `ncu --set full` captures
-    # (profiles/r02_ncu_traffic.json, one record per conv kernel kind, written from the .ncu-rep files of profiles/ncu_target.py)
-    traffic_db = {}
-    try:
-        traffic_db = json.load(open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")))
-    except Exception:
-        pass
-    traffic, traffic_note = None, "no ncu capture of the current kernel committed"
+    peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
+    peak_src = ("MEASURED_PEAKS.json bf16_tflops_sustained" if "bf16_tflops_sustained" in peaks
+                else "H100 SXM data sheet, dense bf16 at 700 W (989 TFLOP/s): not a measured ceiling")
+    step_flop = STEP_GFLOP_PER_IMAGE.get(workload, 0.0) * 1e9 * res["images_per_step"]
+    traffic, traffic_note = None, "no DRAM traffic capture of the current kernels committed"
     roof = {"bound": "tensor", "unit": "TFLOP/s", "peak": peak_tf, "peak_source": peak_src, "traffic": traffic, "traffic_note": traffic_note,
             "step_algorithmic_tflop": step_flop * 1e-12,
             "step_achieved": step_flop / (ms_step * 1e-3) * 1e-12 / world,
             "step_frac": step_flop / (ms_step * 1e-3) * 1e-12 / world / peak_tf}
     CONV_KINDS = ("conv3x3_rows", "conv_fprop_kxk", "conv_fprop_1x1", "conv_wgrad")
     if isinstance(prof, dict) and any(kk in prof for kk in CONV_KINDS):
-        hbm = peaks.get("hbm_gbs", 6500.0)
+        hbm = peaks.get("hbm_gbs", 3350.0)
         # every conv kernel class is listed under roofline.kernels with both of its rates (TFLOP/s and GB/s) and its share of the step
-        kname = {"conv3x3_rows": "conv3x3_rows_kernel (3x3 fprop + dgrad, halo rows, tcgen05)",
-                 "conv_fprop_kxk": "conv_fprop_kernel on k x k filters (fprop + dgrad, tcgen05)",
-                 "conv_fprop_1x1": "conv_fprop_kernel on 1x1 filters / GEMMs (fprop + dgrad, tcgen05; HBM bound)",
-                 "conv_wgrad": "conv_wgrad_kernel + wgrad3x3_c64_kernel (weight gradients, tcgen05)"}
+        kname = {"conv3x3_rows": "conv3x3_rows_kernel (3x3 fprop + dgrad, halo rows, wgmma)",
+                 "conv_fprop_kxk": "conv_fprop_kernel on k x k filters (fprop + dgrad, wgmma)",
+                 "conv_fprop_1x1": "conv_fprop_kernel on 1x1 filters / GEMMs (fprop + dgrad, wgmma; HBM bound)",
+                 "conv_wgrad": "conv_wgrad_kernel + wgrad3x3_c64_kernel (weight gradients, wgmma)"}
         # dominant = the conv kernel class with the most time in the accounting step.  The 1x1 launches of conv_fprop_kernel are
         # HBM bound (K = 32..128 channels: a few FLOP per byte), the others tensor bound; the roofline is reported accordingly.
         dom = max((kk for kk in CONV_KINDS if kk in prof), key=lambda kk: prof[kk]["ms"])
         k = prof[dom]
-        if dom in traffic_db:
-            traffic, traffic_note = traffic_db[dom]["dram_bytes_per_launch"], traffic_db[dom]["note"]
-            roof["traffic_algorithmic_bytes_of_that_launch"] = traffic_db[dom]["algorithmic_bytes"]
-        roof["traffic"], roof["traffic_note"] = traffic, traffic_note
         if dom == "conv_fprop_1x1":
-            roof.update({"bound": "hbm", "unit": "GB/s", "peak": hbm, "peak_source": "MEASURED_PEAKS.json hbm_gbs (copy)"})
+            roof.update({"bound": "hbm", "unit": "GB/s", "peak": hbm,
+                         "peak_source": ("MEASURED_PEAKS.json hbm_gbs (copy)" if "hbm_gbs" in peaks
+                                         else "H100 SXM data sheet HBM3 bandwidth (3.35 TB/s): not a measured ceiling")})
         ew = {kk: vv for kk, vv in prof.items() if kk not in CONV_KINDS and vv.get("gbytes")}
         ew_ms = sum(v["ms"] for v in ew.values())
         ew_gb = sum(v["gbytes"] for v in ew.values())
@@ -581,11 +612,12 @@ def main():
             v, dt, per = cpu_step_images_per_sec(args.config, args.cpu_batch, threads, n_steps=3)
             cpu = {"value": v, "unit": "img/s", "cores": threads, "kind": "port",
                    "sample": "%d of the %d images of each step (2 D updates + 1 G update, fwd+bwd+Adam); 1 warm-up + 3 timed steps, %.1f s; "
-                             "per-step img/s min %.3f max %.3f" % (args.cpu_batch, global_batch, dt, min(per), max(per))}
+                             "per-step img/s min %.3f max %.3f" % (args.cpu_batch, res["images_per_step"], dt, min(per), max(per))}
         except Exception as ex:
             cpu = {"value": None, "unit": "img/s", "cores": threads, "kind": "port", "sample": "failed: %r" % (ex,)}
 
     cfg = config_dict(workload, cfgs, global_batch, world, graphs_wanted(args, per_rank), S, opt.d_updates_per_step, opt.acml_steps)
+    cfg["per_gpu_micro_batch"] = per_rank
     cfg["cuda_graphs_captured"] = res["graphs_captured"]
     cfg["also_measured"] = also
     e2e = res["e2e"]

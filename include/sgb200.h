@@ -1,4 +1,4 @@
-/* libsgb200 — C ABI of the B200-native StudioGAN hot path.
+/* libsgb200 — C ABI of the H100-native StudioGAN hot path.
  *
  * Everything here is plain C: device pointers, sizes, a cudaStream_t passed as void*.  No torch
  * types cross this boundary.  Every entry point returns 0 on success or an SGB_ERR_* code; nothing
@@ -28,14 +28,14 @@ typedef void* sgb_stream_t; /* cudaStream_t */
 
 /* library / device probe: returns the ABI version (or -1), no GPU work. */
 int sgb_abi_version(void);
-/* 0 if a sm_100 device is current and usable, else SGB_ERR_CUDA. */
+/* 0 if a sm_90 device is current and usable, SGB_ERR_UNSUPPORTED on another architecture, else SGB_ERR_CUDA. */
 int sgb_device_check(void);
 /* Make ``device``'s primary context current on the calling host thread (call once per thread that uses the library,
  * e.g. PyTorch autograd worker threads). */
 int sgb_bind_device(int32_t device);
 
 /* ------------------------------------------------------------------------------------------
- * Implicit-GEMM convolution on tcgen05 tensor cores (TMA-staged NHWC tiles, TMEM accumulators).
+ * Implicit-GEMM convolution on Hopper tensor cores (TMA-staged NHWC tiles, wgmma, register accumulators).
  * Stride-1 convolution with KHxKW taps and zero padding; H,W are the OUTPUT spatial size
  * (== input size).  Also serves linear layers (H=W=1) and dgrad (caller passes the
  * transposed/flipped packed weights).
@@ -94,7 +94,7 @@ typedef struct sgb_conv_desc {
 int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream);
 
 /* Weight gradient: dw[co][tap][ci] += sum_{b,h,w} dy[b,h,w,co] * x[b,h+kh-pad,w+kw-pad,ci]
- * (tcgen05 with MN-major operands, split over pixels, fp32 atomics into dw).
+ * (wgmma with MN-major operands, split over pixels, fp32 atomics into dw).
  * Replaces: conv/linear weight-gradient of torch autograd for the same call sites. */
 typedef struct sgb_wgrad_desc {
   int32_t B, H, W;

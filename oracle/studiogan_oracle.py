@@ -656,7 +656,7 @@ def eval_preprocess(images, size=299, quantize=True):
 
 # ---------------------------------------------------------------------------------------------------------------------
 # DCGAN (src/models/deep_conv.py) -- BASELINE config 1, the reference's CPU-only case.  Oracle level only: the product
-# has no sm_100a kernel for the 4x4 / stride-2 (transposed) convolutions (DESIGN.md, out of scope).
+# has no sm_90a kernel for the 4x4 / stride-2 (transposed) convolutions (DESIGN.md, out of scope).
 # ---------------------------------------------------------------------------------------------------------------------
 def dcgan_generator(sd, z, label=None, training=True, track=True):
     """Generator.forward (src/models/deep_conv.py:96-126), unconditional (g_cond_mtd W/O, info N/A):

@@ -1,8 +1,7 @@
-"""Build libsgb200.so (and the bring-up selftest binary) in-tree with nvcc for sm_100a.
+"""Build libsgb200.so (and the bring-up selftest binary) in-tree with nvcc for sm_90a (H100).
 
 Usage: python pytorch-studiogan_b200/build.py [--force] [--selftest]
-The shared library lands in pytorch-studiogan_b200/sgb200/lib/libsgb200.so so that it travels with
-the tree to the GPU box (it is git-ignored, not gpurun-ignored).
+The shared library lands in pytorch-studiogan_b200/sgb200/lib/libsgb200.so (git-ignored build product).
 """
 import hashlib
 import os
@@ -17,7 +16,7 @@ LIBDIR = os.path.join(HERE, "sgb200", "lib")
 LIB = os.path.join(LIBDIR, "libsgb200.so")
 SELFTEST = os.path.join(OBJ, "sgb_selftest")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
 
 

@@ -1,4 +1,4 @@
-// Fused conv epilogue shared by the tcgen05 conv kernels: TMEM accumulator row -> alpha, bias, residual (optionally read
+// Fused conv epilogue shared by the wgmma conv kernels: accumulator row (staged in shared memory) -> alpha, bias, residual (optionally read
 // from a half-resolution tensor = nearest x2 upsample), ReLU, ReLU-mask, post-mask residual -> bf16 / fp32 NHWC store.
 #pragma once
 #include "common.cuh"
@@ -38,7 +38,7 @@ __device__ __forceinline__ uint32_t positive_bits16(const float (&f)[16]) {
 // The same 16 bits from the PACKED bf16 pairs of a post-ReLU piece (every half is +0 or a positive value <= 0x7F80): adding
 // 0x7FFF to a half sets its bit 15 iff it is non-zero without carrying into its neighbour; PRMT gathers the four flag bytes of
 // two words, one multiply moves the four flags into a nibble.  27 integer instructions per piece instead of 40
-// (FSETP + SEL per element + adds) -- the bit plane is paid for by write-bound layers (r02: 1x1 32->128 @256x256 +1.2 ms).
+// (FSETP + SEL per element + adds) -- the bit plane is paid for by write-bound layers.
 __device__ __forceinline__ uint32_t positive_bits16_packed(const uint32_t (&w)[8]) {
   uint32_t bits = 0u;
 #pragma unroll
@@ -66,8 +66,8 @@ __device__ __forceinline__ bool epi_vec_ok(const EpiArgs& p) {
          (p.mask == nullptr || p.mask_cstride % 8 == 0);
 }
 
-// One thread = one accumulator row (TMEM lane).  t_row: TMEM address of this warp's lane quadrant at the accumulator's
-// first column.  All 32 lanes of the warp must call this (tcgen05.ld is warp-collective); stores are predicated by valid.
+// One thread = one accumulator row.  t_row: shared-memory address of this thread's accumulator row (acc_store layout);
+// stores are predicated by valid.
 __device__ __forceinline__ void epilogue_row(const EpiArgs& p, uint32_t t_row, int BN, int n0, bool valid, long long pix,
                                              long long rpix, float alpha, bool vec_ok) {
   const bool res_pre = p.residual != nullptr && !p.res_after;
@@ -75,9 +75,7 @@ __device__ __forceinline__ void epilogue_row(const EpiArgs& p, uint32_t t_row, i
   const float rs = p.res_scale;
   for (int c0 = 0; c0 < BN; c0 += 16) {
     uint32_t v[16];
-    __syncwarp();
-    tmem_ld16(t_row + c0, v);
-    tmem_ld_wait();
+    acc_ld16(t_row + 4u * c0, v);
     const int n = n0 + c0;
     if (!valid || n >= p.Cout) continue;
     float f[16];
@@ -209,12 +207,12 @@ __device__ __forceinline__ bool epi_use_tma(const EpiArgs& p, int BN) {
 
 // Compile-time epilogue variants.  The per-piece loop below runs on 2 warps per scheduler with little latency hiding, so
 // every run-time test of "is there a bias / residual / mask / ragged channel tail" costs issue slots on the critical path of
-// the memory-bound layers (ncu, r01: ~150 SASS instructions per 16-column piece).  F >= 0 fixes those questions at compile
+// the memory-bound layers (~150 SASS instructions per 16-column piece).  F >= 0 fixes those questions at compile
 // time (bit 0 bias, 1 ReLU, 2 residual before the activation, 3 residual after the mask, 4 mask, 5 Cout % 64 == 0 and every
 // 16-byte alignment holds); F < 0 is the fully general run-time version.
 static constexpr int kEpiBias = 1, kEpiRelu = 2, kEpiResPre = 4, kEpiResPost = 8, kEpiMask = 16, kEpiFull = 32;
 // ... bit 6: the mask is a bit plane (mask_bits), 7 / 8: the residual / the bf16 mask tile arrives through the aux TMA ring,
-// 9: the ReLU epilogue also writes its bit plane (relu_bits).  r02 ncu of the fused block-entry dgrad (mask + residual): with these
+// 9: the ReLU epilogue also writes its bit plane (relu_bits).  In the fused block-entry dgrad (mask + residual), with these
 // three questions left to run time the compiler if-converts both sides of each and the piece loop issues 12 instructions per
 // output element (the bias-only variant: 2).
 static constexpr int kEpiMaskBits = 64, kEpiAuxRes = 128, kEpiAuxMask = 256, kEpiBitsOut = 512;
@@ -237,7 +235,7 @@ __host__ __device__ inline int epi_flags_of(const EpiArgs& p) {
 }
 
 // 2^x on the SFU (ex2.approx: 2^-22 relative error, far below the bf16 rounding of the softmax output); the accurate exp2f
-// costs ~10 instructions per element and made the softmax epilogues issue bound (r02: 0.88 ms per score-GEMM pass)
+// costs ~10 instructions per element and made the softmax epilogues issue bound
 __device__ __forceinline__ float fast_ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -255,10 +253,8 @@ __device__ __forceinline__ void epilogue_tile_smstats(const EpiArgs& p, uint32_t
 #pragma unroll 1
     for (int s0 = 0; s0 < 4; s0 += 2) {
       uint32_t v[2][16];
-      __syncwarp();
-      tmem_ld16(t_row + cc * 64 + s0 * 16, v[0]);
-      tmem_ld16(t_row + cc * 64 + (s0 + 1) * 16, v[1]);
-      tmem_ld_wait();
+      acc_ld16(t_row + 4u * (cc * 64 + s0 * 16), v[0]);
+      acc_ld16(t_row + 4u * (cc * 64 + (s0 + 1) * 16), v[1]);
       float pm = -INFINITY;
 #pragma unroll
       for (int q = 0; q < 2; ++q)
@@ -281,107 +277,16 @@ __device__ __forceinline__ void epilogue_tile_smstats(const EpiArgs& p, uint32_t
   }
 }
 
-// Direct-store epilogue of a compile-time variant F >= 0 (bf16 output, Cout % 64 == 0, 16-byte aligned operands): the same
-// arithmetic as epilogue_row without its run-time case analysis, two 16-column pieces per TMEM wait.  Used by the halo-row
-// kernel's second output row at C = 64 (no room for a second staging tile): one full 128-byte line per thread and piece pair.
-template <int F>
-__device__ __forceinline__ void epilogue_row_fast(const EpiArgs& p, uint32_t t_row, int BN, int n0, bool valid, long long pix,
-                                                  long long rpix, float alpha) {
-  static_assert(F >= 0 && (F & kEpiFull), "compile-time variant with a full channel tile");
-  constexpr bool has_bias = (F & kEpiBias) != 0, do_relu = (F & kEpiRelu) != 0, res_pre = (F & kEpiResPre) != 0,
-                 res_post = (F & kEpiResPost) != 0, has_mask = (F & kEpiMask) != 0;
-  const float rs = p.res_scale;
-  bf16* yrow = reinterpret_cast<bf16*>(p.y) + pix * p.y_cstride;
-  for (int c0 = 0; c0 < BN; c0 += 32) {
-    uint32_t v[2][16];
-    __syncwarp();
-    tmem_ld16(t_row + c0, v[0]);
-    tmem_ld16(t_row + c0 + 16, v[1]);
-    tmem_ld_wait();
-    if (!valid || n0 + c0 >= p.Cout) continue;
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      const int n = n0 + c0 + q * 16;
-      float f[16];
-#pragma unroll
-      for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[q][j]) * alpha;
-      if (has_bias) {
-        const float4* bp = reinterpret_cast<const float4*>(p.bias + n);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float4 bb = __ldg(bp + j);
-          f[4 * j + 0] += bb.x; f[4 * j + 1] += bb.y; f[4 * j + 2] += bb.z; f[4 * j + 3] += bb.w;
-        }
-      }
-      if (res_pre || res_post) {
-        // (residual variants are not instantiated for this path today; kept for completeness of the flag set)
-        const uint4* rp = reinterpret_cast<const uint4*>(p.residual + rpix * p.res_cstride + n);
-        if (res_pre) {
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const uint4 r = __ldg(rp + j);
-            f[8 * j + 0] = fmaf(bf16_bits_lo(r.x), rs, f[8 * j + 0]); f[8 * j + 1] = fmaf(bf16_bits_hi(r.x), rs, f[8 * j + 1]);
-            f[8 * j + 2] = fmaf(bf16_bits_lo(r.y), rs, f[8 * j + 2]); f[8 * j + 3] = fmaf(bf16_bits_hi(r.y), rs, f[8 * j + 3]);
-            f[8 * j + 4] = fmaf(bf16_bits_lo(r.z), rs, f[8 * j + 4]); f[8 * j + 5] = fmaf(bf16_bits_hi(r.z), rs, f[8 * j + 5]);
-            f[8 * j + 6] = fmaf(bf16_bits_lo(r.w), rs, f[8 * j + 6]); f[8 * j + 7] = fmaf(bf16_bits_hi(r.w), rs, f[8 * j + 7]);
-          }
-        }
-      }
-      if (do_relu) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) f[j] = fmaxf(f[j], 0.f);
-        if constexpr ((F & kEpiBitsOut) != 0)
-          reinterpret_cast<unsigned short*>(p.relu_bits)[(pix * (p.Cout >> 6) + (n >> 6)) * 4 + ((n >> 4) & 3)] =
-              (unsigned short)positive_bits16(f);
-      }
-      if constexpr (has_mask && (F & kEpiMaskBits) != 0) {
-        apply_bits16(f, __ldg(reinterpret_cast<const unsigned short*>(p.mask_bits) + (pix * (p.Cout >> 6) + (n >> 6)) * 4 + ((n >> 4) & 3)));
-      } else if constexpr (has_mask) {
-        const uint4* mp = reinterpret_cast<const uint4*>(p.mask + pix * p.mask_cstride + n);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const uint4 m = __ldg(mp + j);
-          f[8 * j + 0] = bf16_bits_lo(m.x) > 0.f ? f[8 * j + 0] : 0.f;
-          f[8 * j + 1] = bf16_bits_hi(m.x) > 0.f ? f[8 * j + 1] : 0.f;
-          f[8 * j + 2] = bf16_bits_lo(m.y) > 0.f ? f[8 * j + 2] : 0.f;
-          f[8 * j + 3] = bf16_bits_hi(m.y) > 0.f ? f[8 * j + 3] : 0.f;
-          f[8 * j + 4] = bf16_bits_lo(m.z) > 0.f ? f[8 * j + 4] : 0.f;
-          f[8 * j + 5] = bf16_bits_hi(m.z) > 0.f ? f[8 * j + 5] : 0.f;
-          f[8 * j + 6] = bf16_bits_lo(m.w) > 0.f ? f[8 * j + 6] : 0.f;
-          f[8 * j + 7] = bf16_bits_hi(m.w) > 0.f ? f[8 * j + 7] : 0.f;
-        }
-      }
-      if (res_post) {
-        const uint4* rp = reinterpret_cast<const uint4*>(p.residual + rpix * p.res_cstride + n);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const uint4 r = __ldg(rp + j);
-          f[8 * j + 0] = fmaf(bf16_bits_lo(r.x), rs, f[8 * j + 0]); f[8 * j + 1] = fmaf(bf16_bits_hi(r.x), rs, f[8 * j + 1]);
-          f[8 * j + 2] = fmaf(bf16_bits_lo(r.y), rs, f[8 * j + 2]); f[8 * j + 3] = fmaf(bf16_bits_hi(r.y), rs, f[8 * j + 3]);
-          f[8 * j + 4] = fmaf(bf16_bits_lo(r.z), rs, f[8 * j + 4]); f[8 * j + 5] = fmaf(bf16_bits_hi(r.z), rs, f[8 * j + 5]);
-          f[8 * j + 6] = fmaf(bf16_bits_lo(r.w), rs, f[8 * j + 6]); f[8 * j + 7] = fmaf(bf16_bits_hi(r.w), rs, f[8 * j + 7]);
-        }
-      }
-      uint4* yp = reinterpret_cast<uint4*>(yrow + n);
-      yp[0] = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
-      yp[1] = make_uint4(pack_bf16x2(f[8], f[9]), pack_bf16x2(f[10], f[11]), pack_bf16x2(f[12], f[13]), pack_bf16x2(f[14], f[15]));
-    }
-  }
-}
-
-// t_row : TMEM address (lane quadrant of this warp, first column of the accumulator).
+// t_row : shared-memory address of this thread's accumulator row (first column of the accumulator).
 // c1..c3: box coordinates (w0, h0, b0) of the tile in the output tensor map; channel coordinate = n0 + chunk * 64.
 // stage : this team's staging buffer (1024-byte aligned).  team in {0,1}; row = accumulator row of this thread.
-// NH: warps per (team, lane quadrant).  1: a thread converts all four 16-column pieces of its row of the chunk; 2: two warps share
-// the row (``half`` 0 / 1 takes pieces 0-1 / 2-3), a team is 8 warps -- twice the warps per scheduler to hide the TMEM-load /
-// shared-memory latencies of the per-piece chain (r02 ncu of a 1x1 launch: 3 warps per scheduler, one eligible 46 % of cycles).
-template <int F, int NH = 1>
+// A thread converts all four 16-column pieces of its row of the chunk; a team is 4 warps.
+template <int F>
 __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtensorMap* tmY, uint32_t t_row, int BN, int n0,
                                                   int c1, int c2, int c3, bool valid, long long pix, long long rpix, float alpha,
                                                   uint32_t stage, int team, int row, bool leader, int chunk_stride = 2,
-                                                  const EpiAux* aux = nullptr, uint32_t* sbuf = nullptr, int nbuf = 2, int half = 0) {
-  constexpr int kTeamThreads = 128 * NH;
-  const int sbeg = half * (4 / NH), send = sbeg + 4 / NH;
+                                                  const EpiAux* aux = nullptr, uint32_t* sbuf = nullptr, int nbuf = 2) {
+  constexpr int kTeamThreads = 128;
   constexpr bool sm_apply = F >= 0 && (F & kEpiSmApply) != 0, sm_bwd = F >= 0 && (F & kEpiSmBwd) != 0;
   constexpr float kLog2e = 1.4426950408889634f;
   float sm_a = 0.f, sm_b = 1.f;                    // apply: (row max, 1 / row sum); backward: (delta, -)
@@ -418,12 +323,8 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
     if (nbase >= p.Cout) break;
     uint32_t mlo = 0u, mhi = 0u, olo = 0u, ohi = 0u;
     if (use_mbits && valid) {                    // 8 bytes instead of a 128-byte line of the bf16 activation
-      if (NH == 1) {
-        const uint2 m = __ldg(reinterpret_cast<const uint2*>(p.mask_bits) + pix * nw + (nbase >> 6));
-        mlo = m.x; mhi = m.y;
-      } else {
-        mlo = mhi = __ldg(reinterpret_cast<const uint32_t*>(p.mask_bits) + (pix * nw + (nbase >> 6)) * 2 + half);
-      }
+      const uint2 m = __ldg(reinterpret_cast<const uint2*>(p.mask_bits) + pix * nw + (nbase >> 6));
+      mlo = m.x; mhi = m.y;
     }
     const uint32_t stage_cur = stage + (sbuf ? *sbuf * kEpiStageBytes : 0u);
     const uint32_t srow = stage_cur + (uint32_t)row * 128u;
@@ -442,9 +343,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
       arow_addr = aux->ring + aslot * kEpiStageBytes + (uint32_t)aux->arow * 128u;
       *aux->cnt += 1u;
     }
-    // compile-time variants handle two 16-column pieces per iteration: both TMEM loads are in flight before the single wait
-    // (the variants use ~77 registers, the general version 102), which hides part of the LDTM latency that two warps per
-    // scheduler cannot hide by themselves
+    // compile-time variants handle two 16-column pieces per iteration: both accumulator loads are in flight together
     constexpr int NP = F >= 0 ? 2 : 1;
     auto piece = [&](const int s, const uint32_t (&v)[16], const uint32_t mb) -> uint32_t {
         const int n = nbase + s * 16;
@@ -535,12 +434,10 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
         return ob;
     };
 #pragma unroll 1
-    for (int s0 = sbeg; s0 < send; s0 += NP) {
+    for (int s0 = 0; s0 < 4; s0 += NP) {
       uint32_t v[NP][16];
-      __syncwarp();
 #pragma unroll
-      for (int q = 0; q < NP; ++q) tmem_ld16(t_row + cc * 64 + (s0 + q) * 16, v[q]);
-      tmem_ld_wait();
+      for (int q = 0; q < NP; ++q) acc_ld16(t_row + 4u * (cc * 64 + (s0 + q) * 16), v[q]);
 #pragma unroll
       for (int q = 0; q < NP; ++q) {
         const int s = s0 + q;
@@ -550,8 +447,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
       }
     }
     if (emit_bits && valid) {
-      if (NH == 1) reinterpret_cast<uint2*>(p.relu_bits)[pix * nw + (nbase >> 6)] = make_uint2(olo, ohi);
-      else reinterpret_cast<uint32_t*>(p.relu_bits)[(pix * nw + (nbase >> 6)) * 2 + half] = half ? ohi : olo;
+      reinterpret_cast<uint2*>(p.relu_bits)[pix * nw + (nbase >> 6)] = make_uint2(olo, ohi);
     }
     fence_proxy_async_smem();                    // generic-proxy smem writes -> visible to the TMA (async proxy)
     named_bar_sync(1 + team, kTeamThreads);

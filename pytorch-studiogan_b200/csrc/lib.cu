@@ -9,8 +9,8 @@ extern "C" int sgb_device_check(void) {
   int major = 0, minor = 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return SGB_ERR_CUDA;
   if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) return SGB_ERR_CUDA;
-  if (major != 10) {
-    fprintf(stderr, "[sgb200] device is sm_%d%d; this library is built for sm_100a only\n", major, minor);
+  if (major != 9 || minor != 0) {
+    fprintf(stderr, "[sgb200] device is sm_%d%d; this library is built for sm_90a only\n", major, minor);
     return SGB_ERR_UNSUPPORTED;
   }
   return SGB_OK;

@@ -10,7 +10,7 @@
 // One building block: a 64 x 64 output tile per CTA (256 threads, 4 x 4 register micro-tile each), operands staged through
 // shared memory in 16-deep slices, double-precision FMA.  These are CUDA-core fp64 kernels: the arithmetic must track the
 // host fp64 reference (threshold comparisons in PRDC, a 2048^2 covariance feeding a matrix square root in FID), and
-// Blackwell's tensor pipe has no fp64 advantage to offer here.
+// Hopper's tensor pipe has no fp64 advantage to offer here.
 #include "common.cuh"
 
 namespace sgb {

@@ -1,5 +1,5 @@
 // Stride-2 helpers for the DCGAN layers (src/models/deep_conv.py:20,140: ConvTranspose2d / Conv2d with kernel 4, stride 2,
-// padding 1), which run on the stride-1 tcgen05 conv engine through two exact identities:
+// padding 1), which run on the stride-1 wgmma conv engine through two exact identities:
 //   conv_transpose(x, W; k4 s2 p1)  =  conv_same(zero_stuff(x), W~; k4, taps offset -2..+1)      zero_stuff: y[2h,2w] = x[h,w]
 //   conv(x, W; k4 s2 p1)            =  subsample(conv_same(x, W; k4, taps offset -1..+2))        subsample:  y[h,w] = x[2h,2w]
 // The sub-sampling is the conv engine's own out_sub = 2 store mode; its adjoint -- needed for the strided conv's gradients

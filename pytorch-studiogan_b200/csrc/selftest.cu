@@ -1,4 +1,4 @@
-// Stand-alone bring-up harness for the tcgen05 conv engine: runs on the GPU box without Python.
+// Stand-alone bring-up harness for the wgmma conv engine: runs on the GPU without Python.
 // Compares sgb_conv_fprop / sgb_conv_wgrad with a scalar host loop on small seeded cases, prints layout
 // probes (delta inputs) so a descriptor mistake can be read off the log, and times a few BigGAN-Deep
 // shaped layers.  Bring-up tooling only; the judged parity tests live in tests/ and go through Python.

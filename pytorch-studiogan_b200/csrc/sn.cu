@@ -269,10 +269,10 @@ __global__ void __launch_bounds__(256) sn_pack_batch_kernel(const sgb_sn_layer* 
                                                              bf16* __restrict__ pack_d) {
   // Tile = 32 output channels x 32 input channels x all taps, staged in shared memory so that the fp32 reads (one run of
   // 32*taps floats per output channel) AND both bf16 writes are contiguous: the fprop pack [co][tap][ci] in runs of 32 ci,
-  // the dgrad pack [ci][taps-1-tap][co] in runs of 32 co.  (The element-wise version scattered 2-byte stores: 0.5 ms/call.)
+  // the dgrad pack [ci][taps-1-tap][co] in runs of 32 co.  (The element-wise version scattered 2-byte stores.)
   // Work decomposition: ONE global tile index over all layers (table[l].tile_start = tiles of the layers before l; layers
   // with more than 9 taps count 4096-element pseudo tiles); a block owns a contiguous range of it.  The former
-  // (max tiles) x (layers) grid launched ~300 k blocks of which most returned at once: 0.49 ms per call (r02 launch list).
+  // (max tiles) x (layers) grid launched ~300 k blocks of which most returned at once: most of the call's time.
   constexpr int kT = 32, kMaxTaps = 9;
   __shared__ bf16 tile[kT][kT * kMaxTaps + 2];
   // (total_tiles / tile_start count WORK UNITS of ~1024 weights: a tile of a k-tap layer is k units, a pseudo tile 4, so

@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution / linear / dgrad / wgrad on Blackwell tensor cores.
+// Implicit-GEMM convolution / linear / dgrad / wgrad on Hopper tensor cores (wgmma).
 //
 //   fprop : D[pixel, co]   = sum_{tap, ci}  X[pixel + tap, ci] * Wp[co, tap, ci]
 //           A = X  tile, TMA 4-D box (64 ch, tw, th, nb) over NHWC   -> smem [128 px][64 ch], K-major, SWIZZLE_128B
@@ -7,9 +7,10 @@
 //   wgrad : D[co, ci]      = sum_{pixel}    dY[pixel, co] * X[pixel + tap, ci]           (one tap per work item)
 //           A = dY tile(s), B = X tile(s): same boxes, consumed as MN-major operands (the pixel axis is K).
 //
-// One persistent CTA per SM, 6 warps: warp 0 = TMA producer (one lane), warp 1 = tcgen05.mma issuer (one lane) and
-// TMEM owner, warps 2..5 = epilogue (TMEM -> registers -> fused epilogue -> global).  Two TMEM accumulator stages so
-// the epilogue of tile i overlaps the main loop of tile i+1.
+// One persistent CTA per SM, 3 warpgroups: warp 0 = TMA producer (one lane), warp 2 = auxiliary-operand producer (fprop),
+// warpgroups 1 and 2 = consumers.  Each consumer warpgroup owns 64 of the tile's 128 rows (wgmma M = 64) with its
+// accumulators in registers.  fprop: the consumers stage the finished accumulator tile in shared memory as fp32 rows and
+// then run the fused epilogue on it (one thread = one row); the producer meanwhile fills the operand ring for the next tile.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -18,23 +19,24 @@
 
 namespace sgb {
 
-static constexpr int kWgradThreads = 192;                // wgrad: warps 0 producer, 1 MMA, 2..5 epilogue
-#ifndef SGB_FPROP_NH
-#define SGB_FPROP_NH 1                               // warps per (team, lane quadrant) in the epilogue; 2 = 16 epilogue warps (A/B on one box, r02: 565.1 vs 563.2 ms/step -- no gain, the 1x1 launches sit on the HBM read/write mix, not on epilogue latency)
-#endif
-static constexpr int kFpropNH = SGB_FPROP_NH;
-static constexpr int kFpropEpiThreads = 256 * kFpropNH;   // 2 teams x 4 lane quadrants x NH column halves
-static constexpr int kThreads = 128 + kFpropEpiThreads;  // warps 0..3: producer / MMA / aux producer / (idle), warps 4..19: epilogue teams
-static constexpr int kTileM = 128;          // pixels (fprop) or output channels (wgrad) per tile = TMEM lanes
+static constexpr int kConsumerThreads = 256;              // two consumer warpgroups, M = 64 rows each
+static constexpr int kConsumerWarps = kConsumerThreads / 32;
+static constexpr int kThreads = 128 + kConsumerThreads;   // warpgroup 0: producers (warps 0 / 2), warpgroups 1..2: MMA + epilogue
+static constexpr int kWgradThreads = kThreads;
+static constexpr int kTileM = 128;          // pixels (fprop) or output channels (wgrad) per tile
 static constexpr int kBlockK = 64;          // bf16 elements per 128-byte swizzle row
 static constexpr int kABytes = kTileM * kBlockK * 2;  // 16 KiB
+static constexpr uint32_t kAccBar = 3;      // named barrier of the 256 consumer threads (1, 2: epilogue teams)
+
+// fp32 accumulator staging rows: BN columns + 16 bytes of padding (see acc_store)
+__host__ __device__ inline uint32_t acc_row_bytes(int BN) { return (uint32_t)BN * 4u + 16u; }
 
 struct FpropArgs {
   int B, H, W, Cin, Cout, taps, KW, pad_h, pad_w;
   int tw, th, nb;                 // tile box: tw*th*nb == 128
   int tiles_w, tiles_h, tiles_b, tiles_n, num_tiles;
   int kblocks;                    // ceil(Cin / 64)
-  int BN;                         // output-channel tile (multiple of 16, <= 256)
+  int BN;                         // output-channel tile: 16, 32, 64 or 128
   int w_mode;                     // 0: shared weights [Cout][taps][Cin]; 1: per-image [B][N][K]; 2: per-image MN-major [B][K][N]
   int stages;
   int use_tma;                    // epilogue through staging tiles + TMA tensor stores
@@ -43,30 +45,71 @@ struct FpropArgs {
   int aux_kind, aux_tw, aux_th;   // residual (1) / mask (2) tile staged by TMA; its box is aux_tw x aux_th x nb pixels
   int aux_depth;                  // aux tiles per epilogue team (ring filled by the aux producer warp)
   int out_sub;                    // 2: store only even (h, w) outputs at (h/2, w/2) -> stride-2 convolution (Inception reduction blocks)
-  uint32_t tmem_cols;
   EpiArgs e;
 };
+
+// Main loop of one fprop tile for this consumer warpgroup (rows 64 wg .. 64 wg + 63), then its accumulators -> shared memory.
+template <int BN>
+__device__ __forceinline__ void fprop_mma_tile(const FpropArgs& p, uint32_t smem_base, uint32_t stage_bytes, uint32_t bres_base,
+                                               uint32_t b_bytes, uint32_t bar_base, uint32_t& it, int wg, uint32_t acc_base) {
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  const bool b_mn = (p.w_mode == 2);
+  const int kiters = p.taps * p.kblocks;
+  const uint32_t lane = threadIdx.x & 31;
+  int prev = -1;
+  for (int k = 0; k < kiters; ++k, ++it) {
+    const int s = it % p.stages;
+    const uint32_t ph = (it / p.stages) & 1;
+    mbar_wait(bar_base + 8u * s, ph);
+    const uint32_t sa = smem_base + s * stage_bytes;
+    const uint64_t adesc = make_sdesc_sw128(sa + (uint32_t)wg * 8192u, 16, 1024);   // rows 64 wg.. of [128][64]
+    // K-major B: rows = output channels, +32 B per 16-wide K step.
+    // MN-major B: (BN/64) atoms of [64 k-rows][64 n] 8 KiB apart (LBO), 8-row groups 1 KiB apart (SBO), +2 KiB per K step.
+    const uint32_t sb = p.b_resident ? bres_base + (uint32_t)k * b_bytes : sa + kABytes;     // k = tap * kblocks + kb
+    wgmma_fence();
+    if (b_mn) {
+      const uint64_t bdesc = make_sdesc_sw128(sb, 8192, 1024);
+#pragma unroll
+      for (int kk = 0; kk < kBlockK / 16; ++kk) Wgmma<BN>::template mma<0, 1>(acc, adesc + 2 * kk, bdesc + 128 * kk, (k > 0 || kk > 0) ? 1u : 0u);
+    } else {
+      const uint64_t bdesc = make_sdesc_sw128(sb, 16, 1024);
+#pragma unroll
+      for (int kk = 0; kk < kBlockK / 16; ++kk) Wgmma<BN>::template mma<0, 0>(acc, adesc + 2 * kk, bdesc + 2 * kk, (k > 0 || kk > 0) ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();                          // the previous K block's MMAs have retired: its ring slot is free
+    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev)); }
+    prev = s;
+  }
+  wgmma_wait<0>();
+  acc_fence(acc);
+  __syncwarp();
+  if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev));
+  named_bar_sync(kAccBar, kConsumerThreads);  // every consumer is done reading the previous tile's staged accumulators
+  acc_store<BN>(acc, acc_base + (uint32_t)wg * 64u * acc_row_bytes(BN), acc_row_bytes(BN));
+  named_bar_sync(kAccBar, kConsumerThreads);
+}
 
 template <int F>      // epilogue variant (conv_epilogue.cuh: kEpi* bits fixed at compile time; -1 = run-time flags)
 __global__ void __launch_bounds__(kThreads, 1)
 conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmAux, const FpropArgs p) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t epi_stage_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // two 16 KiB staging tiles when use_tma
-  const uint32_t aux_stage_base = epi_stage_base + (p.use_tma ? 2u * p.epi_nbuf * kEpiStageBytes : 0u);   // + two aux tiles when aux_kind
+  const uint32_t epi_stage_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // staging tiles when use_tma
+  const uint32_t aux_stage_base = epi_stage_base + (p.use_tma ? 2u * p.epi_nbuf * kEpiStageBytes : 0u);   // + aux tiles when aux_kind
   const uint32_t b_bytes = (uint32_t)p.BN * kBlockK * 2;  // same size for K-major [BN][64] and MN-major (BN/64) x [64][64]
   const uint32_t bres_base = aux_stage_base + (p.aux_kind ? 2u * p.aux_depth * kEpiStageBytes : 0u);     // resident weight tiles [tap][kb]
-  const uint32_t smem_base = bres_base + (p.b_resident ? (uint32_t)(p.taps * p.kblocks) * b_bytes : 0u);
+  const uint32_t acc_base = bres_base + (p.b_resident ? (uint32_t)(p.taps * p.kblocks) * b_bytes : 0u);  // fp32 accumulator rows
+  const uint32_t smem_base = acc_base + (uint32_t)kTileM * acc_row_bytes(p.BN);   // 1024-aligned: 128 rows x (16 mod 1024) B
   const uint32_t stage_bytes = kABytes + (p.b_resident ? 0u : b_bytes);  // multiple of 1024 because BN % 8 == 0 -> b_bytes % 1024 == 0
   const uint32_t bar_base = smem_base + (uint32_t)p.stages * stage_bytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * p.stages + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * p.stages + 2 + a); };
-  const uint32_t holder = bar_base + 8u * (2 * p.stages + 4);
-  const uint32_t bres_bar = bar_base + 8u * (2 * p.stages + 6);
-  auto aux_full = [&](int team, int slot) { return bar_base + 8u * (2 * p.stages + 8 + team * p.aux_depth + slot); };
-  auto aux_empty = [&](int team, int slot) { return bar_base + 8u * (2 * p.stages + 8 + (2 + team) * p.aux_depth + slot); };
+  const uint32_t bres_bar = bar_base + 8u * (2 * p.stages);
+  auto aux_full = [&](int team, int slot) { return bar_base + 8u * (2 * p.stages + 1 + team * p.aux_depth + slot); };
+  auto aux_empty = [&](int team, int slot) { return bar_base + 8u * (2 * p.stages + 1 + (2 + team) * p.aux_depth + slot); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -76,28 +119,15 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), kConsumerWarps);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), kFpropEpiThreads);
+    for (int a = 0; a < 2; ++a)
       for (int sl = 0; sl < p.aux_depth; ++sl) { mbar_init(aux_full(a, sl), 1); mbar_init(aux_empty(a, sl), 1); }
-    }
     mbar_init(bres_bar, 1);
     fence_barrier_init();
     if (p.use_tma) tma_prefetch_desc(&tmY);
   }
-  if (warp == 1) {
-    tmem_alloc(holder, p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(holder));
-
-  const int kiters = p.taps * p.kblocks;
 
   if (warp == 0) {
     if (lane == 0) {
@@ -138,40 +168,6 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ------------------------------------------------------------- MMA issuer
-      const bool b_mn = (p.w_mode == 2);
-      const uint32_t idesc = make_idesc_bf16(kTileM, p.BN, 0, b_mn ? 1 : 0);
-      uint32_t it = 0, tcount = 0;
-      if (p.b_resident) { mbar_wait(bres_bar, 0); tc_fence_after(); }
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tcount) {
-        const uint32_t a = tcount & 1, aph = (tcount >> 1) & 1;
-        mbar_wait(tempty_bar(a), aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + a * p.BN;
-        for (int k = 0; k < kiters; ++k, ++it) {
-          const int s = it % p.stages;
-          const uint32_t ph = (it / p.stages) & 1;
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after();
-          const uint32_t sa = smem_base + s * stage_bytes;
-          const uint64_t adesc = make_sdesc_sw128(sa, 16, 1024);
-          // K-major B: rows = output channels, +32 B per 16-wide K step.
-          // MN-major B: (BN/64) atoms of [64 k-rows][64 n] 8 KiB apart (LBO), 8-row groups 1 KiB apart (SBO), +2 KiB per K step.
-          const uint32_t sb = p.b_resident ? bres_base + (uint32_t)k * b_bytes : sa + kABytes;     // k = tap * kblocks + kb
-          const uint64_t bdesc = b_mn ? make_sdesc_sw128(sb, 8192, 1024) : make_sdesc_sw128(sb, 16, 1024);
-          const uint32_t bstep = b_mn ? 128u : 2u;
-#pragma unroll
-          for (int kk = 0; kk < kBlockK / 16; ++kk) {
-            // A: advance 16 bf16 = 32 bytes along K inside the swizzle row: +2 in the (addr >> 4) field
-            umma_f16_ss(d_tmem, adesc + 2 * kk, bdesc + bstep * kk, idesc, (k > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(empty_bar(s));  // smem slot reusable once these MMAs retire
-        }
-        umma_commit(tfull_bar(a));    // accumulator complete
-      }
-    }
   } else if (warp == 2) {
     if (lane == 0 && p.aux_kind) {
       // ------------------------------------------------------------- aux producer: residual / mask boxes, in the order the
@@ -198,25 +194,27 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
     }
   } else if (warp >= 4) {
-    // --------------------------------------------------------------- epilogue: 16 warps, TMEM lane quadrant = warp % 4;
-    // team = which 64-channel chunks (even / odd), half = which two of the four 16-column pieces of a chunk
-    const int q = warp & 3;
-    const int team = ((warp - 4) >> 2) & 1;
-    const int half = (warp - 4) >> 3;
+    // --------------------------------------------------------------- consumers: MMA, then the epilogue on the staged tile.
+    // Epilogue: team = which 64-channel chunks (even / odd) = consumer warpgroup, q = which 32 rows.
+    const int ct = threadIdx.x - 128;
+    const int wg = ct >> 7;
+    const int q = (ct >> 5) & 3;
+    const int team = wg;
     const int row = q * 32 + lane;
-    const bool leader = (q == 0) && (lane == 0) && (half == 0);
+    const bool leader = (q == 0) && (lane == 0);
     const int wi = row % p.tw, hi = (row / p.tw) % p.th, bi = row / (p.tw * p.th);
     const bool vec_ok = epi_vec_ok(p.e);
     const float alpha = p.e.alpha_ptr ? p.e.alpha * __ldg(p.e.alpha_ptr) : p.e.alpha;
     const uint32_t stage = epi_stage_base + team * p.epi_nbuf * kEpiStageBytes;
-    uint32_t aux_cnt = 0, sbuf = 0;
+    const uint32_t t_row = acc_base + (uint32_t)row * acc_row_bytes(p.BN);
+    uint32_t aux_cnt = 0, sbuf = 0, it = 0;
     EpiAux aux;
     aux.kind = p.aux_kind; aux.ring = aux_stage_base + (uint32_t)(team * p.aux_depth) * kEpiStageBytes;
     aux.full0 = aux_full(team, 0); aux.empty0 = aux_empty(team, 0); aux.depth = p.aux_depth; aux.cnt = &aux_cnt;
     const bool aux_half = p.aux_kind == 1 && p.e.res_up2;
     aux.arow = aux_half ? ((bi * p.aux_th + (p.aux_th == p.th ? hi : (hi >> 1))) * p.aux_tw + (wi >> 1)) : row;
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tcount) {
+    if (p.b_resident) mbar_wait(bres_bar, 0);
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       int t = tile;
       const int nt = t % p.tiles_n; t /= p.tiles_n;
       const int wt = t % p.tiles_w; t /= p.tiles_w;
@@ -229,29 +227,22 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                                            : ((long long)b * ((p.H + 1) >> 1) + (h >> 1)) * ((p.W + 1) >> 1) + (w >> 1);
       const long long rpix = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1)) : pix;
 
-      const uint32_t a = tcount & 1, aph = (tcount >> 1) & 1;
-      mbar_wait(tfull_bar(a), aph);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + a * p.BN;
+      switch (p.BN) {
+        case 16: fprop_mma_tile<16>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+        case 32: fprop_mma_tile<32>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+        case 64: fprop_mma_tile<64>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+        default: fprop_mma_tile<128>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+      }
       if constexpr (F >= 0 && (F & kEpiSmStats) != 0) {
-        if (half == 0) epilogue_tile_smstats(p.e, t_row, p.BN, n0, valid, pix, alpha, team, nt * 2 + team);
+        epilogue_tile_smstats(p.e, t_row, p.BN, n0, valid, pix, alpha, team, nt * 2 + team);
       } else if (p.use_tma) {
-        epilogue_tile_tma<F, kFpropNH>(p.e, &tmY, t_row, p.BN, n0, wt * p.tw, ht * p.th, bt * p.nb, valid, pix, rpix, alpha, stage, team, row,
-                             leader, 2, p.aux_kind ? &aux : nullptr, p.epi_nbuf >= 2 ? &sbuf : nullptr, p.epi_nbuf, half);
-      } else if (team == 0 && half == 0) {
+        epilogue_tile_tma<F>(p.e, &tmY, t_row, p.BN, n0, wt * p.tw, ht * p.th, bt * p.nb, valid, pix, rpix, alpha, stage, team, row,
+                             leader, 2, p.aux_kind ? &aux : nullptr, p.epi_nbuf >= 2 ? &sbuf : nullptr, p.epi_nbuf);
+      } else if (team == 0) {
         epilogue_row(p.e, t_row, p.BN, n0, valid, pix, rpix, alpha, vec_ok);
       }
-      tc_fence_before();
-      mbar_arrive(tempty_bar(a));
     }
     if (p.use_tma && leader) bulk_wait_all();   // staging tiles must outlive the last tensor store
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
   }
 }
 
@@ -266,32 +257,104 @@ struct WgradArgs {
   int splits, tiles_per_split;               // K-splits inside a group
   int num_items;                             // tiles_m*tiles_n*taps*groups*splits
   int stages;
-  uint32_t tmem_cols;
   float* dw;
   long long dw_group_stride;
   float* dbias;                              // optional: sum over pixels of dy (bias gradient), from a constant-ones B operand
 };
 
+// work item -> (m tile, n tile, tap, split); n fastest so neighbouring CTAs share the dY tiles in L2
+__device__ __forceinline__ void wgrad_decode(const WgradArgs& p, int item, int& mt, int& nt, int& tap, int& grp, int& pt_begin,
+                                             int& pt_end) {
+  int t = item;
+  nt = t % p.tiles_n; t /= p.tiles_n;
+  tap = t % p.taps; t /= p.taps;
+  mt = t % p.tiles_m; t /= p.tiles_m;
+  const int sp = t % p.splits; t /= p.splits;
+  grp = t;
+  const int g0 = grp * p.tiles_per_group;
+  pt_begin = g0 + sp * p.tiles_per_split;
+  pt_end = min(pt_begin + p.tiles_per_split, g0 + p.tiles_per_group);
+}
+
+// One wgrad work item for this consumer warpgroup (output channels mt*128 + 64 wg ..): MMAs over the item's pixel tiles, then
+// fp32 red.adds straight from the accumulator registers.
+template <int BN>
+__device__ __forceinline__ void wgrad_item(const WgradArgs& p, int item, uint32_t smem_base, uint32_t stage_bytes, uint32_t bar_base,
+                                           uint32_t ones_base, uint32_t& it, int wg) {
+  int mt, nt, tap, grp, pb, pe;
+  wgrad_decode(p, item, mt, nt, tap, grp, pb, pe);
+  const uint32_t lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  const uint32_t a_bytes = 2 * kABytes;
+  float acc[BN / 2], bacc[4];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) bacc[i] = 0.f;
+  // bias gradient: the (first input-channel tile, first tap) items also multiply dY^T by a block of ones (K-major, N = 8)
+  const bool with_bias = p.dbias != nullptr && nt == 0 && tap == 0;
+  const uint64_t ones_desc = make_sdesc_sw128(ones_base, 16, 1024);
+  int prev = -1;
+  for (int pt = pb; pt < pe; ++pt, ++it) {
+    const int s = it % p.stages;
+    const uint32_t ph = (it / p.stages) & 1;
+    mbar_wait(bar_base + 8u * s, ph);
+    const uint32_t sa = smem_base + s * stage_bytes;
+    // MN-major: 64-wide MN atoms are kABytes apart (LBO), 8-row K groups are 1024 B apart (SBO); this warpgroup's M atom = wg
+    const uint64_t adesc = make_sdesc_sw128(sa + (uint32_t)wg * kABytes, kABytes, 1024);
+    const uint64_t bdesc = make_sdesc_sw128(sa + a_bytes, kABytes, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kTileM / 16; ++kk)      // 16 pixels (K) = two 8-row groups = 2048 bytes -> +128 in the (addr >> 4) field
+      Wgmma<BN>::template mma<1, 1>(acc, adesc + 128 * kk, bdesc + 128 * kk, 1u);
+    if (with_bias) {
+#pragma unroll
+      for (int kk = 0; kk < kTileM / 16; ++kk) Wgmma<8>::template mma<1, 0>(bacc, adesc + 128 * kk, ones_desc, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev)); }
+    prev = s;
+  }
+  wgmma_wait<0>();
+  acc_fence(acc);
+  acc_fence(bacc);
+  if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev)); }
+  if (pe <= pb) return;
+  const int co0 = mt * 128 + wg * 64 + (int)(16u * w + (lane >> 2));
+  const int ci0 = nt * BN + 2 * (int)(lane & 3);
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int co = co0 + 8 * hr;
+    if (co >= p.Cout) continue;
+    float* dst = p.dw + grp * p.dw_group_stride + ((long long)co * p.taps + tap) * p.Cin;
+    if (with_bias && (lane & 3) == 0) atomicAdd(p.dbias + co, bacc[2 * hr]);   // column 0 of the ones-product
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int ci = ci0 + 8 * j + e;
+        if (ci < p.Cin) atomicAdd(dst + ci, acc[4 * j + 2 * hr + e]);
+      }
+  }
+}
+
 __global__ void __launch_bounds__(kWgradThreads, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, const WgradArgs p) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t ones_base = (smem_u32(smem_raw) + 1023u) & ~1023u;          // 16 KiB of bf16 1.0 when dbias (any swizzle of ones is ones)
-  const uint32_t smem_base = ones_base + (p.dbias ? (uint32_t)kABytes : 0u);
+  const uint32_t ones_base = (smem_u32(smem_raw) + 1023u) & ~1023u;          // bf16 1.0 slab when dbias
+  const uint32_t smem_base = ones_base + (p.dbias ? 1024u : 0u);
   const uint32_t a_bytes = 2 * kABytes;                       // two 64-channel boxes -> M = 128
   const uint32_t b_bytes = (uint32_t)(p.BN / 64) * kABytes;   // BN/64 boxes
   const uint32_t stage_bytes = a_bytes + b_bytes;
   const uint32_t bar_base = smem_base + (uint32_t)p.stages * stage_bytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * p.stages + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * p.stages + 2 + a); };
-  const uint32_t holder = bar_base + 8u * (2 * p.stages + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   if (p.dbias) {
-    for (uint32_t i = threadIdx.x; i < (uint32_t)kABytes / 16u; i += kWgradThreads)
+    for (uint32_t i = threadIdx.x; i < 1024u / 16u; i += kWgradThreads)
       st_shared_v4(ones_base + i * 16u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u);
     fence_proxy_async_smem();                 // generic-proxy writes -> visible to the tensor core's operand reads
   }
@@ -300,43 +363,18 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
     tma_prefetch_desc(&tmX);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 128);
+      mbar_init(empty_bar(s), kConsumerWarps);
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(holder, p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(holder));
-
-  // work item -> (m tile, n tile, tap, split); n fastest so neighbouring CTAs share the dY tiles in L2
-  auto decode = [&](int item, int& mt, int& nt, int& tap, int& grp, int& pt_begin, int& pt_end) {
-    int t = item;
-    nt = t % p.tiles_n; t /= p.tiles_n;
-    tap = t % p.taps; t /= p.taps;
-    mt = t % p.tiles_m; t /= p.tiles_m;
-    const int sp = t % p.splits; t /= p.splits;
-    grp = t;
-    const int g0 = grp * p.tiles_per_group;
-    pt_begin = g0 + sp * p.tiles_per_split;
-    pt_end = min(pt_begin + p.tiles_per_split, g0 + p.tiles_per_group);
-  };
 
   if (warp == 0) {
     if (lane == 0) {
       uint32_t it = 0;
       for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
         int mt, nt, tap, grp, pb, pe;
-        decode(item, mt, nt, tap, grp, pb, pe);
+        wgrad_decode(p, item, mt, nt, tap, grp, pb, pe);
         const int dh = tap / p.KW - p.pad_h, dw = tap % p.KW - p.pad_w;
         for (int pt = pb; pt < pe; ++pt, ++it) {
           int t = pt;
@@ -356,98 +394,17 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(kTileM, p.BN, 1, 1);  // both operands MN-major
-      const uint32_t idesc_ones = make_idesc_bf16(kTileM, 16, 1, 1);
-      const uint64_t ones_desc = make_sdesc_sw128(ones_base, kABytes, 1024);
-      uint32_t it = 0, tcount = 0;
-      for (int item = blockIdx.x; item < p.num_items; item += gridDim.x, ++tcount) {
-        int mt, nt, tap, grp, pb, pe;
-        decode(item, mt, nt, tap, grp, pb, pe);
-        const uint32_t a = tcount & 1, aph = (tcount >> 1) & 1;
-        mbar_wait(tempty_bar(a), aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + a * p.BN;
-        // bias gradient: the (first input-channel tile, first tap) items also multiply dY^T by a block of ones
-        const bool with_bias = p.dbias != nullptr && nt == 0 && tap == 0;
-        const uint32_t d_bias = tmem_base + 2 * p.BN + a * 16;
-        for (int pt = pb; pt < pe; ++pt, ++it) {
-          const int s = it % p.stages;
-          const uint32_t ph = (it / p.stages) & 1;
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after();
-          const uint32_t sa = smem_base + s * stage_bytes;
-          // MN-major: 64-wide MN atoms are kABytes apart (LBO), 8-row K groups are 1024 B apart (SBO)
-          const uint64_t adesc = make_sdesc_sw128(sa, kABytes, 1024);
-          const uint64_t bdesc = make_sdesc_sw128(sa + a_bytes, kABytes, 1024);
-#pragma unroll
-          for (int kk = 0; kk < kTileM / 16; ++kk) {
-            // 16 pixels (K) = two 8-row groups = 2048 bytes -> +128 in the (addr >> 4) field
-            umma_f16_ss(d_tmem, adesc + 128 * kk, bdesc + 128 * kk, idesc, (pt > pb || kk > 0) ? 1u : 0u);
-          }
-          if (with_bias) {
-#pragma unroll
-            for (int kk = 0; kk < kTileM / 16; ++kk)
-              umma_f16_ss(d_bias, adesc + 128 * kk, ones_desc + 128 * kk, idesc_ones, (pt > pb || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(empty_bar(s));
-        }
-        umma_commit(tfull_bar(a));
-      }
+  } else if (warp >= 4) {
+    const int wg = (threadIdx.x - 128) >> 7;
+    uint32_t it = 0;
+    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
+      if (p.BN == 64) wgrad_item<64>(p, item, smem_base, stage_bytes, bar_base, ones_base, it, wg);
+      else wgrad_item<128>(p, item, smem_base, stage_bytes, bar_base, ones_base, it, wg);
     }
-  } else {
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    uint32_t tcount = 0;
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x, ++tcount) {
-      int mt, nt, tap, grp, pb, pe;
-      decode(item, mt, nt, tap, grp, pb, pe);
-      const int co = mt * 128 + row;
-      const uint32_t a = tcount & 1, aph = (tcount >> 1) & 1;
-      mbar_wait(tfull_bar(a), aph);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + a * p.BN;
-      float* dst = p.dw + grp * p.dw_group_stride + ((long long)co * p.taps + tap) * p.Cin;
-      if (p.dbias != nullptr && nt == 0 && tap == 0) {      // warp-uniform: column 0 of the ones-product = sum over this item's pixels
-        uint32_t v[16];
-        __syncwarp();
-        tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + 2 * p.BN + a * 16, v);
-        tmem_ld_wait();
-        if (pe > pb && co < p.Cout) atomicAdd(p.dbias + co, __uint_as_float(v[0]));
-      }
-      for (int c0 = 0; c0 < p.BN; c0 += 16) {
-        uint32_t v[16];
-        __syncwarp();
-        tmem_ld16(t_row + c0, v);
-        tmem_ld_wait();
-        if (pe <= pb || co >= p.Cout) continue;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int ci = nt * p.BN + c0 + j;
-          if (ci < p.Cin) atomicAdd(dst + ci, __uint_as_float(v[j]));
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(tempty_bar(a));
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
   }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-static inline uint32_t pow2_cols(int need) {
-  uint32_t c = 32;
-  while ((int)c < need) c <<= 1;
-  return c;
-}
-
 // Tile box over (W, H, B) with tw*th*nb == 128. Power-of-two splits; edges are masked / zero-filled.
 static void pick_tile(int H, int W, int B, int& tw, int& th, int& nb) {
   tw = 1;
@@ -520,30 +477,19 @@ static int launch_fprop(int grid, size_t smem, cudaStream_t stream, const CUtens
   return SGB_OK;
 }
 
-static int pick_bn(const sgb_conv_desc* d, long long pixel_tiles) {
+static int pick_bn(const sgb_conv_desc* d) {
   int BN;
   if (d->Cout <= 16) BN = 16;
   else if (d->Cout <= 32) BN = 32;
   else if (d->Cout <= 64) BN = 64;
-  else if (d->Cout <= 128 || d->Cout % 256 != 0) BN = 128;
-  else BN = 256;
-  // 128-wide N tiles only when both halves of every 256-wide tile find an idle SM: an N = 128 tile takes nearly as long as an
-  // N = 256 one (the MMA is bound by the shared-memory fetch of the A tile: 712 vs 1381 TFLOP/s on 3x3 128 / 256 channels), so
-  // splitting pays only while tiles256 <= SMs / 2 (r02, B = 32: 3x3 256->256 @32x32 ran 557 TFLOP/s as 512 N = 128 tiles)
-  {
-    long long tiles256 = pixel_tiles * ((d->Cout + 255) / 256);
-    if (BN == 256 && 2LL * tiles256 <= sm_count()) BN = 128;
-  }
+  else BN = 128;      // 128 x 128 fp32 accumulators: 64 registers per consumer thread, 66 KiB of staging rows
   if (d->w_mode == 2 && BN < 64) BN = 64;  // MN-major B is staged in 64-wide atoms
   return BN;
 }
 
 extern "C" int sgb_conv_softmax_parts(const sgb_conv_desc* d) {
   if (!d || d->Cout <= 0) return 0;
-  int tw, th, nb;
-  pick_tile(d->H, d->W, d->B, tw, th, nb);
-  const long long pixel_tiles = (long long)((d->W + tw - 1) / tw) * ((d->H + th - 1) / th) * ((d->B + nb - 1) / nb);
-  const int BN = pick_bn(d, pixel_tiles);
+  const int BN = pick_bn(d);
   return 2 * ((d->Cout + BN - 1) / BN);
 }
 
@@ -585,7 +531,7 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   p.tiles_w = (d->W + p.tw - 1) / p.tw;
   p.tiles_h = (d->H + p.th - 1) / p.th;
   p.tiles_b = (d->B + p.nb - 1) / p.nb;
-  const int BN = pick_bn(d, p.tiles_w * p.tiles_h * p.tiles_b);
+  const int BN = pick_bn(d);
   p.BN = BN;
   p.w_mode = d->w_mode;
   p.tiles_n = (d->Cout + BN - 1) / BN;
@@ -620,7 +566,8 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   const int nbuf_want = switches().epi_nbuf < 1 ? 1 : (switches().epi_nbuf > 4 ? 4 : switches().epi_nbuf);
   p.epi_nbuf = (p.use_tma && kt <= 2) ? nbuf_want : 1;
   p.aux_depth = p.aux_kind ? (switches().aux_depth < 1 ? 1 : (switches().aux_depth > 3 ? 3 : switches().aux_depth)) : 1;
-  auto ring_kb = [&](int nbuf) { return 216 - (p.use_tma ? 32 * nbuf : 0) - (p.aux_kind ? 32 * p.aux_depth : 0) - (p.b_resident ? (int)(kt * b_tile / 1024) : 0); };
+  const int acc_kb = (int)(kTileM * acc_row_bytes(BN) / 1024);
+  auto ring_kb = [&](int nbuf) { return 216 - acc_kb - (p.use_tma ? 32 * nbuf : 0) - (p.aux_kind ? 32 * p.aux_depth : 0) - (p.b_resident ? (int)(kt * b_tile / 1024) : 0); };
   // keep >= 3 operand ring stages: give back aux depth first, then staging tiles
   while (p.aux_kind && p.aux_depth > 1 && ring_kb(p.epi_nbuf) * 1024 < (int)(3 * stage_bytes)) --p.aux_depth;
   while (p.epi_nbuf > 1 && ring_kb(p.epi_nbuf) * 1024 < (int)(3 * stage_bytes)) --p.epi_nbuf;
@@ -628,7 +575,6 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   if (stages > 8) stages = 8;
   if (stages < 2) stages = 2;
   p.stages = stages;
-  p.tmem_cols = pow2_cols(2 * BN);
   fill_epi(p.e, d);
   p.e.sm_parts = 2 * p.tiles_n;
 
@@ -666,7 +612,8 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
     if (rc) return rc;
   }
   const size_t smem = (size_t)stages * stage_bytes + (p.use_tma ? 2 * p.epi_nbuf * kEpiStageBytes : 0) + (p.aux_kind ? 2 * p.aux_depth * kEpiStageBytes : 0) +
-                      (p.b_resident ? (size_t)kt * b_tile : 0) + 1024 + 8 * (2 * stages + 8 + 4 * 3) + 16;
+                      (p.b_resident ? (size_t)kt * b_tile : 0) + (size_t)kTileM * acc_row_bytes(BN) + 1024 + 8 * (2 * stages + 1 + 4 * 3);
+  SGB_REQUIRE(smem <= 227u * 1024u);
   int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
   // the hot epilogue shapes of the training step get compile-time variants; everything else takes the general kernel
   int f = p.use_tma ? epi_flags_of(p.e) : -1;
@@ -728,8 +675,8 @@ extern "C" int sgb_conv_wgrad(const sgb_wgrad_desc* d, sgb_stream_t stream_) {
   p.dw_group_stride = (long long)d->Cout * p.taps * d->Cin;
   const int base_items = p.tiles_m * p.tiles_n * p.taps * p.groups;
   // K-splits: the persistent grid runs ceil(items / SMs) rounds of one item (= tiles_per_split pixel tiles + a drain) each, so
-  // pick the split count that minimises rounds x (tiles_per_split + drain); r02 ncu: 9 taps x 33 splits = 297 items ran as
-  // 148 + 148 + 1 and left the SMs idle for a third of the launch.
+  // pick the split count that minimises rounds x (tiles_per_split + drain): a last round with a handful of items leaves most
+  // SMs idle.
   {
     const int sms = sm_count();
     const int max_splits = p.tiles_per_group < (4 * sms + base_items - 1) / base_items ? p.tiles_per_group : (4 * sms + base_items - 1) / base_items;
@@ -745,7 +692,6 @@ extern "C" int sgb_conv_wgrad(const sgb_wgrad_desc* d, sgb_stream_t stream_) {
     }
     // near-ties go to MORE splits: concurrent items of one split read the same dY / X tiles at the same moment (36 CTAs on
     // one set of L2 lines for a 256 -> 256 filter), more splits = more distinct streams and drains hidden behind the next item
-    // (r02: 3x3 512->512 @16x16 ran 807 TF/s with 1 split x 144 items and 968 TF/s with 3 x 144)
     for (int s = best + 1; s <= (max_splits < 1 ? 1 : max_splits); ++s) {
       const int tps = (p.tiles_per_group + s - 1) / s;
       const int eff = (p.tiles_per_group + tps - 1) / tps;
@@ -757,10 +703,9 @@ extern "C" int sgb_conv_wgrad(const sgb_wgrad_desc* d, sgb_stream_t stream_) {
   }
   p.num_items = base_items * p.splits;
   const uint32_t stage_bytes = 2 * kABytes + (p.BN / 64) * kABytes;
-  int stages = (int)(((d->dbias ? 224 - 16 : 200) * 1024) / stage_bytes);   // the ones slab must not cost a pipeline stage
+  int stages = (int)((216 * 1024) / stage_bytes);
   if (stages > 6) stages = 6;
   p.stages = stages;
-  p.tmem_cols = pow2_cols(2 * p.BN + (d->dbias ? 32 : 0));
   p.dw = d->dw;
   p.dbias = d->dbias;
   if (d->dbias && !d->accumulate) SGB_CUDA(cudaMemsetAsync(d->dbias, 0, sizeof(float) * (size_t)d->Cout, stream));
@@ -774,7 +719,7 @@ extern "C" int sgb_conv_wgrad(const sgb_wgrad_desc* d, sgb_stream_t stream_) {
   rc = make_act_tmap(&tmX, d->x, d->B, d->H, d->W, d->Cin, d->x_cstride, p.tw, p.th, p.nb);
   if (rc) return rc;
 
-  const size_t smem = (size_t)stages * stage_bytes + (d->dbias ? kABytes : 0) + 1024 + 8 * (2 * stages + 4) + 16;
+  const size_t smem = (size_t)stages * stage_bytes + (d->dbias ? 1024 : 0) + 1024 + 8 * (2 * stages);
   static bool attr_set = false;
   if (!attr_set) {
     SGB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));

@@ -2,14 +2,15 @@
 // BigGAN-Deep at 128x128 / 256x256, where the generic per-tap kernel is bound by L2 -> smem traffic (each output tile
 // re-fetches its input 9x and the whole filter once).  This variant stages HALO ROWS once and forms all nine taps from
 // shared memory:
-//   work item   = two adjacent output rows x 128 pixels x BN channels (two TMEM accumulators, M = 128 each)
+//   work item   = two adjacent output rows x 128 pixels x BN channels (two register accumulators per consumer warpgroup)
 //   A staging   = 4 input rows (h0-1 .. h0+2) of 130 pixels x 64 channels per K block, one TMA box each
 //                 (OOB rows / columns zero-filled = padding); tap (kh, kw) of output row j reads row buffer kh + j at a
 //                 start address advanced by kw pixels (kw * 128 B): rows stay 128 B apart, and the 128-byte swizzle is a
 //                 function of the absolute shared-memory address, so a row-shifted descriptor addresses exactly what TMA wrote
 //   B staging   = filter taps; RESIDENT in smem for the whole persistent CTA when they fit (C = 64: 72 KiB), else a ring
 //   L2 traffic  = 33 KiB per 128 output pixels at C = 64 (was 216 KiB), 210 KiB at C = 128 (was 576 KiB)
-// Warps: 0 = A producer, 1 = MMA issuer + TMEM owner, 2..5 = epilogue, 6 = B producer.
+// Warps: 0 = A producer, 2 = B producer; warpgroups 1 and 2 = consumers (pixels 0..63 / 64..127 of the row, wgmma M = 64),
+// which stage each output row's accumulators in shared memory and run the fused epilogue on it.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "conv_epilogue.cuh"
@@ -19,14 +20,17 @@ namespace sgb {
 static constexpr int kRowPix = 130;
 static constexpr int kRowLoadBytes = kRowPix * 128;   // 16640
 static constexpr int kRowBufBytes = 17 * 1024;        // 17408, keeps every row buffer 1024-byte aligned
-static constexpr int kRowsThreads = 128 + kEpiThreads;  // warps 0: A producer, 1: MMA, 2: B producer, 3: idle, 4..11: epilogue
+static constexpr int kRowsConsumers = 256;
+static constexpr int kRowsThreads = 128 + kRowsConsumers;  // warps 0: A producer, 2: B producer, 4..11: MMA + epilogue
+static constexpr uint32_t kRowsAccBar = 3;                 // named barrier of the consumers (1, 2: epilogue teams)
+
+__host__ __device__ inline uint32_t rows_acc_ld(int BN) { return (uint32_t)BN * 4u + 16u; }
 
 struct RowsArgs {
   int B, H, W, Cin, Cout;
   int kblocks, BN, tiles_n, segs, hpairs, num_tiles;
   int resident, a_stages, b_stages, bo_mode;
-  int use_tma, epi_bufs;   // TMA-store epilogue; 2 staging tiles: team t owns output row t, 1: team 0 handles both rows
-  uint32_t tmem_cols;
+  int use_tma, epi_bufs;   // TMA-store epilogue; one staging tile per team that has chunks (BN / 64 of them, at most 2)
   EpiArgs e;
 };
 
@@ -36,13 +40,122 @@ __device__ __forceinline__ uint64_t sdesc_rows(uint32_t addr, int bo_mode) {
   return d;
 }
 
+// One work item of a consumer warpgroup: both output rows' MMAs over every K block, accumulators for rows 0 / 1 in acc[0 / 1].
+template <int BN>
+__device__ __forceinline__ void rows_mma_tile(const RowsArgs& p, float (&acc)[2][BN / 2], uint32_t a_base, uint32_t a_stage_bytes,
+                                              uint32_t b_base, uint32_t b_tile_bytes, uint32_t bar_base, int nb, uint32_t& ita,
+                                              uint32_t& itb, int wg) {
+  const uint32_t lane = threadIdx.x & 31;
+  auto a_full = [&](int s) { return bar_base + 8u * s; };
+  auto a_empty = [&](int s) { return bar_base + 8u * (p.a_stages + s); };
+  auto b_full = [&](int s) { return bar_base + 8u * (2 * p.a_stages + s); };
+  auto b_empty = [&](int s) { return bar_base + 8u * (2 * p.a_stages + nb + s); };
+#pragma unroll
+  for (int j = 0; j < 2; ++j)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[j][i] = 0.f;
+  for (int kb = 0; kb < p.kblocks; ++kb, ++ita) {
+    const int sa_i = ita % p.a_stages;
+    mbar_wait(a_full(sa_i), (ita / p.a_stages) & 1);
+    const uint32_t sa = a_base + sa_i * a_stage_bytes + (uint32_t)wg * 8192u;   // this warpgroup's 64 pixels
+    int bprev = -1;                              // filter-ring slot of the previous tap, released once its MMAs retire
+    for (int tap = 0; tap < 9; ++tap) {
+      const int kh = tap / 3, kw = tap % 3;
+      uint32_t sb;
+      int bslot = 0;
+      if (p.resident) {
+        sb = b_base + ((kb * 3 + kw) * 3 + kh) * b_tile_bytes;     // resident order [kb][kw][kh]
+      } else {
+        bslot = itb % p.b_stages;
+        mbar_wait(b_full(bslot), (itb / p.b_stages) & 1);
+        sb = b_base + bslot * b_tile_bytes;
+      }
+      const uint64_t bdesc = make_sdesc_sw128(sb, 16, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const uint64_t adesc = sdesc_rows(sa + (kh + j) * kRowBufBytes + kw * 128, p.bo_mode);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) Wgmma<BN>::template mma<0, 0>(acc[j], adesc + 2 * kk, bdesc + 2 * kk, 1u);
+      }
+      wgmma_commit();
+      if (!p.resident) {
+        wgmma_wait<1>();
+        __syncwarp();
+        if (bprev >= 0 && lane == 0) mbar_arrive(b_empty(bprev));
+        bprev = bslot;
+        ++itb;
+      }
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (bprev >= 0 && lane == 0) mbar_arrive(b_empty(bprev));
+    if (lane == 0) mbar_arrive(a_empty(sa_i));
+  }
+  acc_fence(acc[0]);
+  acc_fence(acc[1]);
+}
+
+// Stages output row j's accumulators of this warpgroup in shared memory (after every consumer is done with the previous ones).
+template <int BN>
+__device__ __forceinline__ void rows_stage(const float (&acc)[BN / 2], uint32_t acc_base, int wg) {
+  named_bar_sync(kRowsAccBar, kRowsConsumers);
+  acc_store<BN>(acc, acc_base + (uint32_t)wg * 64u * rows_acc_ld(BN), rows_acc_ld(BN));
+  named_bar_sync(kRowsAccBar, kRowsConsumers);
+}
+
+template <int F, int BN>
+__device__ __forceinline__ void rows_consumer(const RowsArgs& p, const CUtensorMap* tmY, uint32_t epi_stage_base, uint32_t acc_base,
+                                              uint32_t a_base, uint32_t a_stage_bytes, uint32_t b_base, uint32_t b_tile_bytes,
+                                              uint32_t bar_base, int nb) {
+  const int ct = threadIdx.x - 128;
+  const int wg = ct >> 7, team = wg;
+  const int q = (ct >> 5) & 3;
+  const int lane = threadIdx.x & 31;
+  const int row = q * 32 + lane;
+  const bool leader = (q == 0) && (lane == 0);
+  const bool vec_ok = epi_vec_ok(p.e);
+  const float alpha = p.e.alpha_ptr ? p.e.alpha * __ldg(p.e.alpha_ptr) : p.e.alpha;
+  const uint32_t t_row = acc_base + (uint32_t)row * rows_acc_ld(BN);
+  uint32_t ita = 0, itb = 0;
+  if (p.resident) mbar_wait(bar_base + 8u * (2 * p.a_stages), 0);
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    int t = tile;
+    const int nt = t % p.tiles_n; t /= p.tiles_n;
+    const int ws = t % p.segs; t /= p.segs;
+    const int hp = t % p.hpairs; t /= p.hpairs;
+    const int b = t;
+    float acc[2][BN / 2];
+    rows_mma_tile<BN>(p, acc, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb, ita, itb, wg);
+    const int w = ws * 128 + row;
+#pragma unroll 1
+    for (int j = 0; j < 2; ++j) {
+      if (j == 0) rows_stage<BN>(acc[0], acc_base, wg);    // static indices keep both accumulators in registers
+      else rows_stage<BN>(acc[1], acc_base, wg);
+      const int h = hp * 2 + j;
+      const long long pix = ((long long)b * p.H + h) * p.W + w;
+      const long long rpix = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1)) : pix;
+      if (p.use_tma) {
+        // the two teams take alternate 64-channel chunks of the row, each through its own staging tile
+        if (team < p.epi_bufs)
+          epilogue_tile_tma<F>(p.e, tmY, t_row, BN, nt * BN, ws * 128, h, b, true, pix, rpix, alpha, epi_stage_base + team * kEpiStageBytes,
+                               team, row, leader, 2);
+      } else if (team == 0) {
+        epilogue_row(p.e, t_row, BN, nt * BN, true, pix, rpix, alpha, vec_ok);
+      }
+    }
+  }
+  if (p.use_tma && leader && team < p.epi_bufs) bulk_wait_all();
+}
+
 template <int F>      // epilogue variant, see conv_epilogue.cuh
 __global__ void __launch_bounds__(kRowsThreads, 1)
 conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmY, const RowsArgs p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t epi_stage_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t smem_base = epi_stage_base + (p.use_tma ? (uint32_t)p.epi_bufs * kEpiStageBytes : 0u);
+  const uint32_t acc_base = epi_stage_base + (p.use_tma ? (uint32_t)p.epi_bufs * kEpiStageBytes : 0u);
+  const uint32_t smem_base = acc_base + 128u * rows_acc_ld(p.BN);   // 1024-aligned: 128 rows x (16 mod 1024) B
   const uint32_t a_stage_bytes = 4 * kRowBufBytes;
   const uint32_t b_tile_bytes = (uint32_t)p.BN * 128u;
   const uint32_t a_base = smem_base;
@@ -54,9 +167,6 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   auto a_empty = [&](int s) { return bar_base + 8u * (p.a_stages + s); };
   auto b_full = [&](int s) { return bar_base + 8u * (2 * p.a_stages + s); };
   auto b_empty = [&](int s) { return bar_base + 8u * (2 * p.a_stages + nb + s); };
-  auto tfull = [&](int a) { return bar_base + 8u * (2 * p.a_stages + 2 * nb + a); };
-  auto tempty = [&](int a) { return bar_base + 8u * (2 * p.a_stages + 2 * nb + 2 + a); };
-  const uint32_t holder = bar_base + 8u * (2 * p.a_stages + 2 * nb + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -64,20 +174,11 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int s = 0; s < p.a_stages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), 1); }
-    for (int s = 0; s < nb; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull(a), 1); mbar_init(tempty(a), kEpiThreads); }
+    for (int s = 0; s < p.a_stages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), kRowsConsumers / 32); }
+    for (int s = 0; s < nb; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), kRowsConsumers / 32); }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(holder, p.tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(holder));
 
   auto decode = [&](int tile, int& nt, int& ws, int& hp, int& b) {
     int t = tile;
@@ -109,7 +210,6 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       // ------------------------------------------------------------- B producer: filter taps (resident or ring)
       if (p.resident) {
         mbar_arrive_expect_tx(b_full(0), 9u * p.kblocks * b_tile_bytes);
-        // resident order [kb][kw][kh]: the taps (kh, kw) and (kh + 1, kw) are adjacent, so one N = 2 BN operand covers both
         for (int tap = 0; tap < 9; ++tap)
           for (int kb = 0; kb < p.kblocks; ++kb)
             tma_load_3d(b_base + ((kb * 3 + tap % 3) * 3 + tap / 3) * b_tile_bytes, &tmB, b_full(0), kb * 64, tap, 0);
@@ -128,119 +228,13 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ------------------------------------------------------------- MMA issuer
-      const uint32_t idesc = make_idesc_bf16(128, p.BN, 0, 0);
-      if (p.resident) { mbar_wait(b_full(0), 0); tc_fence_after(); }
-      uint32_t ita = 0, itb = 0, tcount = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tcount) {
-        const uint32_t as = tcount & 1, aph = (tcount >> 1) & 1;
-        mbar_wait(tempty(as), aph ^ 1);
-        tc_fence_after();
-        for (int kb = 0; kb < p.kblocks; ++kb, ++ita) {
-          const int sa_i = ita % p.a_stages;
-          mbar_wait(a_full(sa_i), (ita / p.a_stages) & 1);
-          tc_fence_after();
-          const uint32_t sa = a_base + sa_i * a_stage_bytes;
-          if (p.resident) {
-            // Halo row r feeds output row 1 through tap row r - 1 and output row 0 through tap row r.  For r = 1, 2 both exist:
-            // ONE MMA with B = [W(r-1, kw); W(r, kw)] (N = 2 BN) writes the [row 1 | row 0] accumulator pair, so the A
-            // operand (the dominant shared-memory read at N = 64) is fetched once instead of twice.
-            const uint32_t d_pair = tmem_base + as * 2 * p.BN;
-            const uint32_t idesc2 = make_idesc_bf16(128, 2 * p.BN, 0, 0);
-            for (int r = 1; r <= 2; ++r)
-              for (int kw = 0; kw < 3; ++kw) {
-                const uint64_t bdesc = make_sdesc_sw128(b_base + ((kb * 3 + kw) * 3 + (r - 1)) * b_tile_bytes, 16, 1024);
-                const uint64_t adesc = sdesc_rows(sa + r * kRowBufBytes + kw * 128, p.bo_mode);
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk)
-                  umma_f16_ss(d_pair, adesc + 2 * kk, bdesc + 2 * kk, idesc2, (kb > 0 || r > 1 || kw > 0 || kk > 0) ? 1u : 0u);
-              }
-            for (int e = 0; e < 2; ++e)          // r = 0: tap row 0 -> output row 0;  r = 3: tap row 2 -> output row 1
-              for (int kw = 0; kw < 3; ++kw) {
-                const uint64_t bdesc = make_sdesc_sw128(b_base + ((kb * 3 + kw) * 3 + (e ? 2 : 0)) * b_tile_bytes, 16, 1024);
-                const uint64_t adesc = sdesc_rows(sa + (e ? 3 : 0) * kRowBufBytes + kw * 128, p.bo_mode);
-                const uint32_t d_one = d_pair + (e ? 0 : p.BN);
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) umma_f16_ss(d_one, adesc + 2 * kk, bdesc + 2 * kk, idesc, 1u);
-              }
-            umma_commit(a_empty(sa_i));
-            continue;
-          }
-          for (int tap = 0; tap < 9; ++tap) {          // filter ring (the resident case was handled above)
-            const int kh = tap / 3, kw = tap % 3;
-            const int sb = itb % p.b_stages;
-            mbar_wait(b_full(sb), (itb / p.b_stages) & 1);
-            tc_fence_after();
-            const uint64_t bdesc = make_sdesc_sw128(b_base + sb * b_tile_bytes, 16, 1024);
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-              const uint64_t adesc = sdesc_rows(sa + (kh + j) * kRowBufBytes + kw * 128, p.bo_mode);
-              const uint32_t d_tmem = tmem_base + (as * 2 + j) * p.BN;
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk)
-                umma_f16_ss(d_tmem, adesc + 2 * kk, bdesc + 2 * kk, idesc, (kb > 0 || tap > 0 || kk > 0) ? 1u : 0u);
-            }
-            umma_commit(b_empty(sb));
-            ++itb;
-          }
-          umma_commit(a_empty(sa_i));
-        }
-        umma_commit(tfull(as));
-      }
-    }
   } else if (warp >= 4) {
-    // --------------------------------------------------------------- epilogue: 8 warps (two teams)
-    const int q = warp & 3;
-    const int team = (warp - 4) >> 2;
-    const int row = q * 32 + lane;
-    const bool leader = (q == 0) && (lane == 0);
-    const bool vec_ok = epi_vec_ok(p.e);
-    const float alpha = p.e.alpha_ptr ? p.e.alpha * __ldg(p.e.alpha_ptr) : p.e.alpha;
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tcount) {
-      int nt, ws, hp, b;
-      decode(tile, nt, ws, hp, b);
-      const int w = ws * 128 + row;
-      const uint32_t as = tcount & 1, aph = (tcount >> 1) & 1;
-      mbar_wait(tfull(as), aph);
-      tc_fence_after();
-#pragma unroll 1
-      for (int j = 0; j < 2; ++j) {
-        const int h = hp * 2 + j;
-        const long long pix = ((long long)b * p.H + h) * p.W + w;
-        const long long rpix = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1)) : pix;
-        const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (as * 2 + (p.resident ? 1 - j : j)) * p.BN;
-        if (p.use_tma) {
-          // team t owns output row t.  epi_bufs == 2: both teams stage + TMA-store; epi_bufs == 1 (no room for a second
-          // staging tile, C = 64): team 0 stages + TMA-stores row 0 while team 1 writes row 1 with direct 16-byte stores
-          // (one full 128-byte line per thread at C = 64) -- two rows drain concurrently instead of back to back.
-          if (team == j) {
-            if (p.epi_bufs == 2 || team == 0) {
-              const uint32_t stage = epi_stage_base + ((p.epi_bufs == 2) ? team : 0) * kEpiStageBytes;
-              // one team covers every chunk of its row: run the chunk loop for both parities on the team's own barrier
-              epilogue_tile_tma<F>(p.e, &tmY, t_row, p.BN, nt * p.BN, ws * 128, h, b, true, pix, rpix, alpha, stage, team, row, leader, 1);
-            } else {
-              if constexpr (F >= 0) epilogue_row_fast<F>(p.e, t_row, p.BN, nt * p.BN, true, pix, rpix, alpha);
-              else epilogue_row(p.e, t_row, p.BN, nt * p.BN, true, pix, rpix, alpha, vec_ok);
-            }
-          }
-        } else if (team == 0) {
-          epilogue_row(p.e, t_row, p.BN, nt * p.BN, true, pix, rpix, alpha, vec_ok);
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(tempty(as));
+    switch (p.BN) {
+      case 16: rows_consumer<F, 16>(p, &tmY, epi_stage_base, acc_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
+      case 32: rows_consumer<F, 32>(p, &tmY, epi_stage_base, acc_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
+      case 64: rows_consumer<F, 64>(p, &tmY, epi_stage_base, acc_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
+      default: rows_consumer<F, 128>(p, &tmY, epi_stage_base, acc_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
     }
-    if (p.use_tma && leader) bulk_wait_all();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
   }
 }
 
@@ -269,7 +263,7 @@ int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream, int bo_mode
   RowsArgs p;
   p.B = d->B; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.Cout = d->Cout;
   p.kblocks = d->Cin / 64;
-  p.BN = d->Cout <= 128 ? (d->Cout + 15) / 16 * 16 : 128;   // Cout = 8 (padded image channels) runs as one N = 16 tile
+  p.BN = d->Cout <= 16 ? 16 : d->Cout <= 32 ? 32 : d->Cout <= 64 ? 64 : 128;   // Cout = 8 (padded image channels) runs as one N = 16 tile
   p.tiles_n = (d->Cout + p.BN - 1) / p.BN;
   p.segs = d->W / 128;
   p.hpairs = d->H / 2;
@@ -281,24 +275,20 @@ int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream, int bo_mode
   const uint32_t resident_bytes = 9u * p.kblocks * b_tile;
   p.use_tma = (!d->y_fp32 && p.BN % 64 == 0 && d->y_cstride % 8 == 0 && (!d->residual || d->res_cstride % 8 == 0) &&
                (!d->mask || d->mask_cstride % 8 == 0) && use_tma_env) ? 1 : 0;
-  p.epi_bufs = 2;
-  p.resident = (p.tiles_n == 1 && resident_bytes + 2 * a_stage + (p.use_tma ? kEpiStageBytes : 0) <= budget) ? 1 : 0;
+  p.epi_bufs = p.BN >= 128 ? 2 : 1;
+  const uint32_t fixed = 128u * rows_acc_ld(p.BN) + (p.use_tma ? p.epi_bufs * kEpiStageBytes : 0);
+  p.resident = (p.tiles_n == 1 && resident_bytes + a_stage + fixed <= budget) ? 1 : 0;
   if (p.resident) {
-    if (p.use_tma && resident_bytes + 2 * a_stage + 2 * kEpiStageBytes > budget) p.epi_bufs = 1;
-    const uint32_t epi_bytes = p.use_tma ? p.epi_bufs * kEpiStageBytes : 0;
-    p.a_stages = (int)((budget - resident_bytes - epi_bytes) / a_stage);
+    p.a_stages = (int)((budget - resident_bytes - fixed) / a_stage);
     if (p.a_stages > 3) p.a_stages = 3;
     p.b_stages = 1;
   } else {
     p.a_stages = 2;
-    const uint32_t epi_bytes = p.use_tma ? p.epi_bufs * kEpiStageBytes : 0;
-    p.b_stages = (int)((budget - 2 * a_stage - epi_bytes) / b_tile);
+    if (2 * a_stage + fixed + 2 * b_tile > budget) p.a_stages = 1;
+    p.b_stages = (int)((budget - p.a_stages * a_stage - fixed) / b_tile);
     if (p.b_stages > 6) p.b_stages = 6;
     if (p.b_stages < 2) return SGB_ERR_UNSUPPORTED;
   }
-  uint32_t cols = 32;
-  while ((int)cols < 4 * p.BN) cols <<= 1;
-  p.tmem_cols = cols;
   fill_epi(p.e, d);
 
   CUtensorMap tmA, tmB;
@@ -326,8 +316,9 @@ int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream, int bo_mode
   }
   const int nb = p.resident ? 1 : p.b_stages;
   const size_t smem = (size_t)p.a_stages * a_stage + (p.resident ? resident_bytes : p.b_stages * b_tile) +
-                      (p.use_tma ? p.epi_bufs * kEpiStageBytes : 0) + 1024 +
-                      8 * (2 * p.a_stages + 2 * nb + 4) + 16;
+                      (p.use_tma ? p.epi_bufs * kEpiStageBytes : 0) + 128u * rows_acc_ld(p.BN) + 1024 +
+                      8 * (2 * p.a_stages + 2 * nb);
+  SGB_REQUIRE(smem <= 227u * 1024u);
   const int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
   const int f = p.use_tma ? epi_flags_of(p.e) : -1;
   switch (f) {

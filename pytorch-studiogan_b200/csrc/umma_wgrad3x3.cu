@@ -1,29 +1,27 @@
 // Weight gradient of 3x3 / pad 1 convolutions with 64 input channels (the widest-resolution layers of BigGAN-Deep: the
-// generic wgrad kernel reloads dY and a shifted X tile for every one of the 9 taps and wastes half of each M = 128 MMA
-// when Cout = 64; it runs at 235 TFLOP/s, bound by L2 -> smem traffic).
+// generic wgrad kernel reloads dY and a shifted X tile for every one of the 9 taps).
 //
 //   dW[co][tap][ci] = sum_{b,h,w} dY[b,h,w,co] * X[b,h+dh,w+dw,ci]
 //
 // Formulation (pixels are the contraction dimension, all operands MN-major / SWIZZLE_128B):
 //   A (M side) = X halo: one tile stages 4 halo rows x 130 pixels x 64 channels ONCE; tap (dh,dw) is the same buffer read
-//                from pixel offset (dh+1)*130 + (dw+1).  An M = 128 operand consists of two 64-channel atoms "LBO" bytes
-//                apart -- choosing LBO = the pixel distance between two taps makes ONE MMA produce TWO taps:
-//                D[(tap_pair, ci)][co].  9 taps = 4 pairs + 1 single -> 5 accumulator blocks of 64 columns (320 of 512).
+//                from pixel offset (dh+1)*130 + (dw+1) -- one 64-channel MN atom, M = 64.
 //   B (N side) = dY tile, 2 rows x 128 pixels x Cout (<= 64) channels.
-// Per tile: 2 rows x 5 blocks x 8 MMAs (K = 16 pixels) of 128x64x16 = 2560 tensor cycles for 98.5 KB of loads
-// (38 B/cycle/SM), 90 % of the MMAs' rows useful.  A CTA accumulates its whole pixel range in TMEM and drains once with
-// coalesced fp32 red.adds (lanes = consecutive ci).
+// Three consumer warpgroups, one filter row (kh) each: three taps x 64 x 64 fp32 accumulators in registers per warpgroup,
+// accumulated over the CTA's whole pixel range and drained once with fp32 red.adds.  The bias gradient is one more small
+// product on the first warpgroup: dY^T times a constant-ones operand.
 #include "common.cuh"
 #include "ptx.cuh"
 
 namespace sgb {
 
-static constexpr int kW3Threads = 192;              // warp 0 producer, warp 1 MMA + TMEM owner, warps 2-5 drain
+static constexpr int kW3Consumers = 384;            // warpgroups 1..3: taps (kh, 0..2) for kh = warpgroup - 1
+static constexpr int kW3Threads = 128 + kW3Consumers;   // warp 0 producer
 static constexpr int kW3Px = 128;                   // pixels per tile row
 static constexpr int kW3Halo = kW3Px + 2;           // halo row pitch in pixels
 static constexpr uint32_t kW3DyBytes = 2 * kW3Px * 128;                       // 32 KB
 static constexpr uint32_t kW3XBytes = 4 * kW3Halo * 128;                      // 66 560 B
-static constexpr uint32_t kW3XAlloc = (kW3XBytes + 2048 + 1023) / 1024 * 1024;  // + slack: the unpaired tap's idle atom reads past
+static constexpr uint32_t kW3XAlloc = (kW3XBytes + 1023) / 1024 * 1024;
 static constexpr uint32_t kW3Stage = kW3DyBytes + kW3XAlloc;
 static constexpr int kW3Stages = 2;
 
@@ -33,19 +31,90 @@ struct W3Args {
   int tiles_w, tiles_h;          // tiles per row, row pairs per image
   long long tiles;               // B * tiles_h * tiles_w
   float* dw;
-  float* dbias;                  // optional: sum of dY over all pixels (idle atom of the unpaired tap reads constant ones)
+  float* dbias;                  // optional: sum of dY over all pixels
 };
+
+// Consumer warpgroup of filter row kh: taps (kh, 0..2) over the CTA's tile range, then the red.add drain.  BIAS: this
+// warpgroup also accumulates dY^T times a constant-ones operand (the bias gradient).
+template <bool BIAS>
+__device__ __forceinline__ void w3_consumer(const W3Args& p, uint32_t smem_base, uint32_t ones_base, uint32_t bar_base,
+                                            long long t_begin, long long t_end, int kh) {
+  const int lane = threadIdx.x & 31;
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (kW3Stages + s); };
+  float acc[3][32], bacc[4];
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[k][i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) bacc[i] = 0.f;
+  const uint64_t ones_desc = make_sdesc_sw128(ones_base, 16, 1024);   // K-major N = 8: every element is 1.0
+  uint32_t it = 0;
+  int prev = -1;
+  for (long long t = t_begin; t < t_end; ++t, ++it) {
+    const int s = it % kW3Stages;
+    const uint32_t ph = (it / kW3Stages) & 1;
+    mbar_wait(full_bar(s), ph);
+    const uint32_t ys = smem_base + s * kW3Stage;
+    const uint32_t xs = ys + kW3DyBytes;
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint64_t bdesc = make_sdesc_sw128(ys + (uint32_t)(j * kW3Px) * 128u, 128 * kW3Px, 1024);
+#pragma unroll
+      for (int kw = 0; kw < 3; ++kw) {
+        const uint64_t adesc = make_sdesc_sw128(xs + (uint32_t)((kh + j) * kW3Halo + kw) * 128u, 8192, 1024);
+#pragma unroll
+        for (int kk = 0; kk < kW3Px / 16; ++kk)   // 16 pixels (K) = two 8-row groups = 2048 bytes -> +128 in the (addr >> 4) field
+          Wgmma<64>::mma<1, 1>(acc[kw], adesc + 128 * kk, bdesc + 128 * kk, 1u);
+      }
+      if constexpr (BIAS) {
+#pragma unroll
+        for (int kk = 0; kk < kW3Px / 16; ++kk) Wgmma<8>::mma<1, 0>(bacc, bdesc + 128 * kk, ones_desc, 1u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar(prev)); }
+    prev = s;
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int k = 0; k < 3; ++k) acc_fence(acc[k]);
+  acc_fence(bacc);
+  __syncwarp();
+  if (lane == 0) mbar_arrive(empty_bar(prev));
+  // drain: fragment rows = input channels, columns = output channels
+  const int w = (threadIdx.x >> 5) & 3;
+  const int ci0 = 16 * w + (lane >> 2), co0 = 2 * (lane & 3);
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int ci = ci0 + 8 * hr;
+    if (BIAS && (lane & 3) == 0 && ci < p.Cout) atomicAdd(p.dbias + ci, bacc[2 * hr]);   // bias fragment rows = output channels
+    if (ci >= p.Cin) continue;
+#pragma unroll
+    for (int kw = 0; kw < 3; ++kw) {
+      const int tap = kh * 3 + kw;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int co = co0 + 8 * j + e;
+          if (co < p.Cout) atomicAdd(p.dw + ((long long)co * 9 + tap) * p.dw_cin + ci, acc[kw][4 * j + 2 * hr + e]);
+        }
+    }
+  }
+}
 
 __global__ void __launch_bounds__(kW3Threads, 1)
 wgrad3x3_c64_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, const W3Args p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + kW3Stages * kW3Stage;
+  const uint32_t ones_base = smem_base + kW3Stages * kW3Stage;          // 1 KB of bf16 1.0 (8 rows x 128 B)
+  const uint32_t bar_base = ones_base + 1024u;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kW3Stages + s); };
-  const uint32_t done_bar = bar_base + 8u * (2 * kW3Stages);
-  const uint32_t holder = bar_base + 8u * (2 * kW3Stages + 1);
-  const uint32_t ones_base = (bar_base + 8u * (2 * kW3Stages + 2) + 1023u) & ~1023u;   // 2 KB of bf16 1.0 (16 K rows x 128 B)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -55,25 +124,16 @@ wgrad3x3_c64_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_const
     tma_prefetch_desc(&tmX);
     for (int s = 0; s < kW3Stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), kW3Consumers / 32);
     }
-    mbar_init(done_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(holder, 512);
-    tmem_relinquish();
-  }
   if (p.dbias) {
-    for (int i = threadIdx.x; i < 2048 / 4; i += kW3Threads)
+    for (int i = threadIdx.x; i < 1024 / 4; i += kW3Threads)
       asm volatile("st.shared.u32 [%0], %1;" ::"r"(ones_base + 4u * i), "r"(0x3F803F80u) : "memory");
     fence_proxy_async_smem();                     // the MMA reads this region through the async proxy
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(holder));
 
   // contiguous tile range of this CTA
   const long long t_begin = p.tiles * blockIdx.x / gridDim.x;
@@ -96,82 +156,11 @@ wgrad3x3_c64_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_const
         tma_load_4d(sa + kW3DyBytes, &tmX, full_bar(s), 0, w0 - 1, h0 - 1, b);   // out-of-range halo = zero padding
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && t_end > t_begin) {
-      const uint32_t idesc = make_idesc_bf16(128, 64, 1, 1);   // both operands MN-major
-      uint32_t it = 0;
-      for (long long t = t_begin; t < t_end; ++t, ++it) {
-        const int s = it % kW3Stages;
-        const uint32_t ph = (it / kW3Stages) & 1;
-        mbar_wait(full_bar(s), ph);
-        tc_fence_after();
-        const uint32_t ys = smem_base + s * kW3Stage;
-        const uint32_t xs = ys + kW3DyBytes;
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-#pragma unroll
-          for (int g = 0; g < 5; ++g) {
-            const int tap = 2 * g;
-            const int off = (tap / 3 + j) * kW3Halo + tap % 3;                 // pixel offset of the pair's first tap
-            // second atom = next tap: +1 pixel, or (row + 1, dw = -1) for the pair (tap 2, tap 3): 130 - 2 pixels;
-            // the unpaired tap 8 drags an idle atom one pixel further (rows ignored by the drain, reads stay in the slack)
-            const uint32_t lbo = (tap == 2 ? (uint32_t)(kW3Halo - 2) : 1u) * 128u;
-            const uint32_t a0 = xs + (uint32_t)off * 128u;
-            const uint64_t adesc = make_sdesc_sw128(a0, lbo, 1024);
-            const uint64_t bdesc = make_sdesc_sw128(ys + (uint32_t)(j * kW3Px) * 128u, 128 * kW3Px, 1024);
-            const uint32_t d_tmem = tmem_base + (uint32_t)g * 64u;
-#pragma unroll
-            for (int kk = 0; kk < kW3Px / 16; ++kk) {
-              // 16 pixels (K) = two 8-row groups = 2048 bytes -> +128 in the (addr >> 4) field
-              uint64_t ad = adesc + 128 * kk;
-              // bias gradient for free: the idle second atom of the unpaired tap 8 is pointed (through the LBO) at a
-              // constant-one K slab, so rows 64..127 of its accumulator block receive sum_k dY[k][co]
-              if (g == 4 && p.dbias) ad = make_sdesc_sw128(a0 + 2048u * kk, ones_base - (a0 + 2048u * kk), 1024);
-              umma_f16_ss(d_tmem, ad, bdesc + 128 * kk, idesc, (it > 0 || j > 0 || kk > 0) ? 1u : 0u);
-            }
-          }
-        }
-        umma_commit(empty_bar(s));
-      }
-      umma_commit(done_bar);
-    }
-  } else if (t_end > t_begin) {
-    const int q = warp & 3;
-    const int m = q * 32 + lane;                 // accumulator row = (tap parity, ci)
-    const int ci = m & 63;
-    mbar_wait(done_bar, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int g = 0; g < 5; ++g) {
-      const int tap = 2 * g + (m >> 6);
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)g * 64u;
-#pragma unroll 1
-      for (int c0 = 0; c0 < 64; c0 += 16) {
-        uint32_t v[16];
-        __syncwarp();
-        tmem_ld16(t_row + c0, v);
-        tmem_ld_wait();
-        if (tap == 9 && m == 64 && p.dbias) {          // row (tap 9, ci 0): the bias gradient
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            if (c0 + i < p.Cout) atomicAdd(p.dbias + c0 + i, __uint_as_float(v[i]));
-        }
-        if (tap >= 9 || ci >= p.Cin) continue;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int co = c0 + i;
-          if (co < p.Cout) atomicAdd(p.dw + ((long long)co * 9 + tap) * p.dw_cin + ci, __uint_as_float(v[i]));
-        }
-      }
-    }
-    tc_fence_before();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  } else if (warp >= 4 && t_end > t_begin) {
+    const int kh = (threadIdx.x - 128) >> 7;    // this warpgroup's filter row
+    // the bias product is a compile-time property of the consumer body: a branch between the wgmmas would serialise them
+    if (p.dbias != nullptr && kh == 0) w3_consumer<true>(p, smem_base, ones_base, bar_base, t_begin, t_end, kh);
+    else w3_consumer<false>(p, smem_base, ones_base, bar_base, t_begin, t_end, kh);
   }
 }
 
@@ -196,7 +185,7 @@ int launch_wgrad3x3_c64(const sgb_wgrad_desc* d, cudaStream_t stream) {
     int rc = make_tmap_bf16(&tmDY, d->dy, 4, dims, strides, box);
     if (rc) return rc;
   }
-  const size_t smem = (size_t)kW3Stages * kW3Stage + 1024 + 8 * (2 * kW3Stages + 2) + 1024 + 2048 + 16;
+  const size_t smem = (size_t)kW3Stages * kW3Stage + 1024 + 1024 + 8 * (2 * kW3Stages);
   static bool attr_set = false;
   if (!attr_set) {
     SGB_CUDA(cudaFuncSetAttribute(wgrad3x3_c64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));

@@ -108,7 +108,7 @@ def _direct_grad_ptr(p):
 
 
 def conv_param_grads(x, dz, weight, need_w, need_b, KH, KW, pad, dims, sigma, u_saved, v_saved, perm_S=1, sn_pass=None, bias=None):
-    """Weight and bias gradient of y = conv(x, W / sigma) + b given dz = dL/dy (NHWC bf16): tcgen05 weight-gradient kernel,
+    """Weight and bias gradient of y = conv(x, W / sigma) + b given dz = dL/dy (NHWC bf16): wgmma weight-gradient kernel,
     then the spectral-norm chain rule (sgb_sn_backward).  The weight gradient is added straight into the flat gradient
     arena when the parameter opted in (returns None for it then).  The bias gradient rides on the weight-gradient launch
     (a constant-ones operand on the tensor pipe, sgb_conv_wgrad_fuses_dbias); only a frozen weight with a live bias falls
@@ -846,7 +846,7 @@ FUSED_SOFTMAX = os.environ.get("SGB_ATTN_FUSED_SOFTMAX", "1") != "0"   # A/B swi
 class SelfAttentionFn(TFunction):
     """ops.SelfAttention.forward (src/utils/ops.py:83-103) with the attention map materialised in bf16:
        theta = conv(x), phi = maxpool(conv(x)), g = maxpool(conv(x)); P = softmax(theta . phi^T); o = P . g;
-       out = x + sigma * conv(o).  All contractions run on the tcgen05 engine (batched modes 1/2)."""
+       out = x + sigma * conv(o).  All contractions run on the wgmma engine (batched modes 1/2)."""
 
     @staticmethod
     def forward(ctx, x, w_theta, w_phi, w_g, w_o, sigma, cfgs):

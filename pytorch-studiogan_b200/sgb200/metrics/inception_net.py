@@ -1,4 +1,4 @@
-"""FID InceptionV3 feature extractor on the tcgen05 conv engine (reference ``src/metrics/inception_net.py``).
+"""FID InceptionV3 feature extractor on the wgmma conv engine (reference ``src/metrics/inception_net.py``).
 
 Same network as the reference's ``InceptionV3`` (torchvision ``inception_v3(num_classes=1008, aux_logits=False)`` with the
 TF-compatible pooling variants FIDInceptionA/C/E_1/E_2, :110-249) in inference mode: BatchNorm (eps 1e-3) is folded into the

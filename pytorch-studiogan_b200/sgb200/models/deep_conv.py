@@ -6,7 +6,7 @@ Drop-in for the reference ``src/models/deep_conv.py``: same constructor signatur
   GenBlock  (ref :15-43)    ConvTranspose 4x4 / stride 2 / pad 1 -> BN (or cBN) -> ReLU
   DiscBlock (ref :129-153)  conv 3x3 -> [BN] -> ReLU -> conv 4x4 / stride 2 / pad 1 -> [BN] -> ReLU
 
-Both stride-2 layers run on the stride-1 tcgen05 engine through exact identities (csrc/resample.cu): the transposed
+Both stride-2 layers run on the stride-1 wgmma engine through exact identities (csrc/resample.cu): the transposed
 convolution is a 4x4 same-size convolution of the zero-stuffed input, the strided convolution stores every other output of
 a 4x4 same-size convolution (the engine's out_sub mode).  That spends 4x the minimal FLOPs on those layers -- DCGAN is the
 reference's 0.8 GFLOP CPU-sized config; it is here for completeness of the model API, not for its roofline.

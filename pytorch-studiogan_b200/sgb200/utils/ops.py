@@ -38,7 +38,7 @@ def _w(module):
 
 
 class _ConvBase(nn.Conv2d):
-    """Stride-1 convolution on the tcgen05 engine (3x3 / 1x1 as used by every BigGAN / ResNetGAN block)."""
+    """Stride-1 convolution on the wgmma engine (3x3 / 1x1 as used by every BigGAN / ResNetGAN block)."""
     spectral = False
 
     def __init__(self, in_channels, out_channels, kernel_size, stride=1, padding=0, dilation=1, groups=1, bias=True):

@@ -1,9 +1,9 @@
-"""Generates the golden vectors under tests/golden/ by running the UNMODIFIED reference (imported from
-/root/reference/src) on seeded CPU inputs.  Run in the build container only:
+"""Generates the golden vectors under tests/golden/ by running the UNMODIFIED reference (a PyTorch-StudioGAN checkout;
+SGB_REFERENCE = its src/ directory) on seeded CPU inputs:
 
-    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
+    SGB_REFERENCE=<checkout>/src PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
 
-The reference tree is read-only and absent on the GPU box, so the resulting .npz files are committed next to this
+The tests must not depend on a reference checkout, so the resulting .npz files are committed next to this
 script.  Missing plotting / IO packages of the reference are stubbed (they are not on the hot path), see SURVEY.md A.1.
 """
 import os
@@ -18,7 +18,9 @@ sys.dont_write_bytecode = True
 for name in ["matplotlib", "matplotlib.pyplot", "seaborn", "h5py", "kornia", "kornia.filters", "kornia.geometry",
              "kornia.geometry.transform", "timm", "timm.models", "timm.models.layers"]:
     sys.modules[name] = MagicMock()
-REF = os.environ.get("SGB_REFERENCE", "/root/reference/src")
+REF = os.environ.get("SGB_REFERENCE")
+if not REF or not os.path.isdir(REF):
+    sys.exit("set SGB_REFERENCE to the src/ directory of a PyTorch-StudioGAN checkout")
 sys.path.insert(0, REF)
 
 import torch  # noqa: E402

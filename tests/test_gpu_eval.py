@@ -1,5 +1,5 @@
 """GPU tests of the evaluation path (SURVEY.md 8a rows a18-a24): device pre-processing, Inception conv pipeline on the
-tcgen05 engine, and IS / FID / PRDC computed from its features, against the oracle and the reference goldens."""
+wgmma conv engine, and IS / FID / PRDC computed from its features, against the oracle and the reference goldens."""
 import os
 
 import numpy as np

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  Every test drives the product path — Python modules ->
+"""GPU parity tests (run on an H100: pytest -m gpu).  Every test drives the product path — Python modules ->
 autograd ops -> ctypes -> libsgb200 kernels — and compares with the CPU oracle (oracle/studiogan_oracle.py) or with the
 committed golden vectors produced by the real reference.
 
