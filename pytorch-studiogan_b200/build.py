@@ -1,6 +1,6 @@
-"""Build libsgb200.so (and the bring-up selftest binary) in-tree with nvcc for sm_90a (H100).
+"""Build libsgb200.so in-tree with nvcc for sm_90a (H100).
 
-Usage: python pytorch-studiogan_b200/build.py [--force] [--selftest]
+Usage: python pytorch-studiogan_b200/build.py [--force]
 The shared library lands in pytorch-studiogan_b200/sgb200/lib/libsgb200.so (git-ignored build product).
 """
 import hashlib
@@ -14,14 +14,13 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIBDIR = os.path.join(HERE, "sgb200", "lib")
 LIB = os.path.join(LIBDIR, "libsgb200.so")
-SELFTEST = os.path.join(OBJ, "sgb_selftest")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
 
 
 def _sources():
-    return sorted(f for f in os.listdir(CSRC) if f.endswith(".cu") and f != "selftest.cu")
+    return sorted(f for f in os.listdir(CSRC) if f.endswith(".cu"))
 
 
 def _digest(paths):
@@ -50,7 +49,7 @@ def _compile(src):
     return obj
 
 
-def build(force=False, selftest=False):
+def build(force=False):
     os.makedirs(OBJ, exist_ok=True)
     os.makedirs(LIBDIR, exist_ok=True)
     if force:
@@ -68,15 +67,9 @@ def build(force=False, selftest=False):
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))
         os.replace(tmp, LIB)
-    if selftest:
-        cmd = [NVCC] + FLAGS + [os.path.join(CSRC, "selftest.cu"), "-o", SELFTEST, "-L" + LIBDIR, "-lsgb200",
-                                "-Xlinker", "-rpath", "-Xlinker", "$ORIGIN/../sgb200/lib"]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        if r.returncode != 0:
-            raise RuntimeError("selftest build failed:\n%s\n%s" % (r.stdout, r.stderr))
     return LIB
 
 
 if __name__ == "__main__":
-    lib = build(force="--force" in sys.argv, selftest="--selftest" in sys.argv)
+    lib = build(force="--force" in sys.argv)
     print(lib)

@@ -80,6 +80,27 @@ inline int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const ui
   return 0;
 }
 
+// NHWC bf16 activation [B][H][W][C] with channel stride cstride (elements); box = 64 channels x tw x th x nb pixels.
+inline int make_act_tmap(CUtensorMap* m, const void* base, int B, int H, int W, int C, long long cstride, int tw, int th, int nb) {
+  uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)B};
+  uint64_t strides[3] = {(uint64_t)cstride * 2, (uint64_t)cstride * 2 * W, (uint64_t)cstride * 2 * W * H};
+  uint32_t box[4] = {64, (uint32_t)tw, (uint32_t)th, (uint32_t)nb};
+  return make_tmap_bf16(m, base, 4, dims, strides, box);
+}
+
+// Launches Kernel with the full 227 KiB of opt-in shared memory available; the attribute is set once per kernel.
+template <auto Kernel, typename... Args>
+inline int launch_kernel(int grid, int threads, size_t smem, cudaStream_t stream, const Args&... args) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    SGB_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_set = true;
+  }
+  Kernel<<<grid, threads, smem, stream>>>(args...);
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
 inline int sm_count() {
   static int n = 0;
   if (n) return n;

@@ -11,8 +11,6 @@
 // warpgroups 1 and 2 = consumers.  Each consumer warpgroup owns 64 of the tile's 128 rows (wgmma M = 64) with its
 // accumulators in registers.  fprop: the consumers stage the finished accumulator tile in shared memory as fp32 rows and
 // then run the fused epilogue on it (one thread = one row); the producer meanwhile fills the operand ring for the next tile.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "ptx.cuh"
 #include "conv_epilogue.cuh"
@@ -40,7 +38,7 @@ struct FpropArgs {
   int w_mode;                     // 0: shared weights [Cout][taps][Cin]; 1: per-image [B][N][K]; 2: per-image MN-major [B][K][N]
   int stages;
   int use_tma;                    // epilogue through staging tiles + TMA tensor stores
-  int epi_nbuf;                   // staging tiles per epilogue team (2..4: stores overlap the next chunks' conversion)
+  int epi_nbuf;                   // staging tiles per epilogue team (2: stores overlap the next chunk's conversion)
   int b_resident;                 // 1: every weight tile of this CTA's channel tile stays in shared memory (loaded once)
   int aux_kind, aux_tw, aux_th;   // residual (1) / mask (2) tile staged by TMA; its box is aux_tw x aux_th x nb pixels
   int aux_depth;                  // aux tiles per epilogue team (ring filled by the aux producer warp)
@@ -430,54 +428,8 @@ void fill_epi(EpiArgs& e, const sgb_conv_desc* d) {
   e.sm_mode = d->sm_mode; e.sm_parts = 0; e.sm_stats = d->sm_stats; e.sm_delta = d->sm_delta;
 }
 
-static int make_act_tmap(CUtensorMap* m, const void* base, int B, int H, int W, int C, long long cstride, int tw, int th,
-                         int nb) {
-  uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)B};
-  uint64_t strides[3] = {(uint64_t)cstride * 2, (uint64_t)cstride * 2 * W, (uint64_t)cstride * 2 * W * H};
-  uint32_t box[4] = {64, (uint32_t)tw, (uint32_t)th, (uint32_t)nb};
-  return make_tmap_bf16(m, base, 4, dims, strides, box);
-}
-
-}  // namespace sgb
-
-using namespace sgb;
-
-namespace sgb {
-bool wgrad3x3_c64_eligible(const sgb_wgrad_desc* d);
-int launch_wgrad3x3_c64(const sgb_wgrad_desc* d, cudaStream_t stream);
-bool conv3x3_rows_eligible(const sgb_conv_desc* d);
-int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream, int bo_mode, int use_tma_env);
-}  // namespace sgb
-
-static int env_int(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return v ? atoi(v) : dflt;
-}
-// Bring-up switches: read from the environment ONCE per process (a conv launch used to call getenv five times).
-struct EngineSwitches {
-  int conv3x3_rows, rows_base_offset, epi_tma, epi_tma_maxk, epi_aux, epi_nbuf, wgrad3x3, b_resident, aux_depth;
-};
-static const EngineSwitches& switches() {
-  static const EngineSwitches s = {env_int("SGB_CONV3X3_ROWS", 1), env_int("SGB_ROWS_BASE_OFFSET", 0), env_int("SGB_EPI_TMA", 1),
-                                   env_int("SGB_EPI_TMA_MAXK", 640), env_int("SGB_EPI_AUX", 1), env_int("SGB_EPI_NBUF", 2),
-                                   env_int("SGB_WGRAD3X3", 1), env_int("SGB_B_RESIDENT", 1), env_int("SGB_AUX_DEPTH", 2)};
-  return s;
-}
-
-template <int F>
-static int launch_fprop(int grid, size_t smem, cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmY,
-                        const CUtensorMap& tmAux, const FpropArgs& p) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    SGB_CUDA(cudaFuncSetAttribute(conv_fprop_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  conv_fprop_kernel<F><<<grid, kThreads, smem, stream>>>(tmA, tmB, tmY, tmAux, p);
-  SGB_LAUNCH_CHECK();
-  return SGB_OK;
-}
-
-static int pick_bn(const sgb_conv_desc* d) {
+// Output-channel tile of the fprop kernels (the halo-row kernel takes it too).
+int pick_bn(const sgb_conv_desc* d) {
   int BN;
   if (d->Cout <= 16) BN = 16;
   else if (d->Cout <= 32) BN = 32;
@@ -486,6 +438,18 @@ static int pick_bn(const sgb_conv_desc* d) {
   if (d->w_mode == 2 && BN < 64) BN = 64;  // MN-major B is staged in 64-wide atoms
   return BN;
 }
+
+// The staged TMA-store epilogue pays off on output-heavy layers only: K = taps * Cin up to this bound.
+static constexpr int kEpiTmaMaxK = 640;
+
+bool wgrad3x3_c64_eligible(const sgb_wgrad_desc* d);
+int launch_wgrad3x3_c64(const sgb_wgrad_desc* d, cudaStream_t stream);
+bool conv3x3_rows_eligible(const sgb_conv_desc* d);
+int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream);
+
+}  // namespace sgb
+
+using namespace sgb;
 
 extern "C" int sgb_conv_softmax_parts(const sgb_conv_desc* d) {
   if (!d || d->Cout <= 0) return 0;
@@ -516,13 +480,8 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   SGB_REQUIRE(d->sm_mode != 1 || d->sm_stats);
   SGB_REQUIRE(d->sm_mode != 2 || d->sm_stats);
   SGB_REQUIRE(d->sm_mode != 3 || (d->sm_delta && d->sm_p && d->sm_p_cstride % 8 == 0 && ((uintptr_t)d->sm_p & 15) == 0));
-  {
-    // wide, few-channel 3x3 layers: halo-row kernel (umma_conv3x3.cu).  SGB_CONV3X3_ROWS=0 forces the generic kernel.
-    const EngineSwitches& sw = switches();
-    if (sw.conv3x3_rows && d->Hin <= 0 && d->Win <= 0 && d->out_sub != 2 && conv3x3_rows_eligible(d))
-      return launch_conv3x3_rows(d, stream, sw.rows_base_offset, sw.epi_tma);
-  }
-  SGB_REQUIRE(((uintptr_t)d->bias & 15) == 0 && ((uintptr_t)d->residual & 15) == 0 && ((uintptr_t)d->mask & 15) == 0);
+  // wide, few-channel 3x3 layers: halo-row kernel (umma_conv3x3.cu)
+  if (d->Hin <= 0 && d->Win <= 0 && d->out_sub != 2 && conv3x3_rows_eligible(d)) return launch_conv3x3_rows(d, stream);
 
   FpropArgs p;
   p.B = d->B; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.Cout = d->Cout;
@@ -542,10 +501,10 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   SGB_REQUIRE(p.out_sub == 1 || (!d->residual && !d->mask));
   p.use_tma = (p.out_sub == 1 && !d->y_fp32 && BN % 64 == 0 && d->Cout % 8 == 0 && d->y_cstride % 8 == 0 &&
                (!d->residual || d->res_cstride % 8 == 0) && (!d->mask || d->mask_cstride % 8 == 0) &&
-               p.taps * d->Cin <= switches().epi_tma_maxk && switches().epi_tma) ? 1 : 0;   // output-heavy layers only
+               p.taps * d->Cin <= kEpiTmaMaxK) ? 1 : 0;
   // auxiliary epilogue operand through TMA: exactly one of residual / mask, bf16 NHWC with 16-byte aligned channel stride
   p.aux_kind = 0; p.aux_tw = p.tw; p.aux_th = p.th;
-  if (p.use_tma && switches().epi_aux && (d->residual != nullptr || d->mask != nullptr)) {   // (mask_bits are 8-byte direct loads)
+  if (p.use_tma && (d->residual != nullptr || d->mask != nullptr)) {   // (mask_bits are 8-byte direct loads)
     // one operand rides TMA: the mask when both are present (full-resolution tile; the residual of such launches is the
     // quarter-size pooled-skip gradient, whose direct 16-byte loads are shared by 2x2 pixel neighbours through L1)
     if (d->mask) p.aux_kind = 2;
@@ -561,11 +520,10 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   // space of the B halves of the ring buys more staging tiles per epilogue team = more store bytes in flight
   const uint32_t b_tile = (uint32_t)BN * kBlockK * 2;
   const int kt = p.taps * p.kblocks;
-  p.b_resident = (switches().b_resident && d->w_mode == 0 && p.tiles_n == 1 && kt <= 2 && kt * b_tile <= 64u * 1024u) ? 1 : 0;
+  p.b_resident = (d->w_mode == 0 && p.tiles_n == 1 && kt <= 2 && kt * b_tile <= 64u * 1024u) ? 1 : 0;
   const uint32_t stage_bytes = kABytes + (p.b_resident ? 0u : b_tile);
-  const int nbuf_want = switches().epi_nbuf < 1 ? 1 : (switches().epi_nbuf > 4 ? 4 : switches().epi_nbuf);
-  p.epi_nbuf = (p.use_tma && kt <= 2) ? nbuf_want : 1;
-  p.aux_depth = p.aux_kind ? (switches().aux_depth < 1 ? 1 : (switches().aux_depth > 3 ? 3 : switches().aux_depth)) : 1;
+  p.epi_nbuf = (p.use_tma && kt <= 2) ? 2 : 1;
+  p.aux_depth = p.aux_kind ? 2 : 1;
   const int acc_kb = (int)(kTileM * acc_row_bytes(BN) / 1024);
   auto ring_kb = [&](int nbuf) { return 216 - acc_kb - (p.use_tma ? 32 * nbuf : 0) - (p.aux_kind ? 32 * p.aux_depth : 0) - (p.b_resident ? (int)(kt * b_tile / 1024) : 0); };
   // keep >= 3 operand ring stages: give back aux depth first, then staging tiles
@@ -621,7 +579,7 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   if (f >= 0 && p.aux_kind == 1) f |= kEpiAuxRes;
   if (f >= 0 && p.aux_kind == 2) f |= kEpiAuxMask;
 #define SGB_FPROP_CASE(FLAGS) \
-  case (FLAGS): return launch_fprop<(FLAGS)>(grid, smem, stream, tmA, tmB, tmY, tmAux, p);
+  case (FLAGS): return launch_kernel<conv_fprop_kernel<(FLAGS)>>(grid, kThreads, smem, stream, tmA, tmB, tmY, tmAux, p);
   switch (f) {
     SGB_FPROP_CASE(kEpiFull)                                                          // dgrad / attention GEMMs
     SGB_FPROP_CASE(kEpiFull | kEpiBias)                                               // generator convs
@@ -638,14 +596,14 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
     SGB_FPROP_CASE(kEpiFull | kEpiSmStats)                                            // attention: row (max, sum exp) partials of theta . phi^T
     SGB_FPROP_CASE(kEpiFull | kEpiSmApply)                                            // attention: P = softmax(theta . phi^T) written directly
     SGB_FPROP_CASE(kEpiFull | kEpiSmBwd)                                              // attention: dS = P * (do . g^T - delta)
-    default: return launch_fprop<-1>(grid, smem, stream, tmA, tmB, tmY, tmAux, p);
+    default: return launch_kernel<conv_fprop_kernel<-1>>(grid, kThreads, smem, stream, tmA, tmB, tmY, tmAux, p);
   }
 #undef SGB_FPROP_CASE
 }
 
 extern "C" int sgb_conv_wgrad_fuses_dbias(const sgb_wgrad_desc* d) {
   if (!d) return 0;
-  if (switches().wgrad3x3 && wgrad3x3_c64_eligible(d)) return 1;
+  if (wgrad3x3_c64_eligible(d)) return 1;
   return d->per_image ? 0 : 1;          // generic kernel: constant-ones B operand on its (first channel tile, first tap) items
 }
 
@@ -655,7 +613,7 @@ extern "C" int sgb_conv_wgrad(const sgb_wgrad_desc* d, sgb_stream_t stream_) {
   SGB_REQUIRE(d->B > 0 && d->H > 0 && d->W > 0 && d->Cin > 0 && d->Cout > 0 && d->KH > 0 && d->KW > 0);
   SGB_REQUIRE(d->Cin % 8 == 0 && d->x_cstride % 8 == 0 && d->Cout % 8 == 0 && d->dy_cstride % 8 == 0);
   SGB_REQUIRE(((uintptr_t)d->x & 15) == 0 && ((uintptr_t)d->dy & 15) == 0);
-  if (switches().wgrad3x3 && wgrad3x3_c64_eligible(d)) return launch_wgrad3x3_c64(d, stream);
+  if (wgrad3x3_c64_eligible(d)) return launch_wgrad3x3_c64(d, stream);
   SGB_REQUIRE(d->dbias == nullptr || !d->per_image);
 
   WgradArgs p;
@@ -720,13 +678,6 @@ extern "C" int sgb_conv_wgrad(const sgb_wgrad_desc* d, sgb_stream_t stream_) {
   if (rc) return rc;
 
   const size_t smem = (size_t)stages * stage_bytes + (d->dbias ? 1024 : 0) + 1024 + 8 * (2 * stages);
-  static bool attr_set = false;
-  if (!attr_set) {
-    SGB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
   int grid = p.num_items < sm_count() ? p.num_items : sm_count();
-  conv_wgrad_kernel<<<grid, kWgradThreads, smem, stream>>>(tmDY, tmX, p);
-  SGB_LAUNCH_CHECK();
-  return SGB_OK;
+  return launch_kernel<conv_wgrad_kernel>(grid, kWgradThreads, smem, stream, tmDY, tmX, p);
 }

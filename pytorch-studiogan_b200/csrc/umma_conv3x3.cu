@@ -29,16 +29,10 @@ __host__ __device__ inline uint32_t rows_acc_ld(int BN) { return (uint32_t)BN * 
 struct RowsArgs {
   int B, H, W, Cin, Cout;
   int kblocks, BN, tiles_n, segs, hpairs, num_tiles;
-  int resident, a_stages, b_stages, bo_mode;
+  int resident, a_stages, b_stages;
   int use_tma, epi_bufs;   // TMA-store epilogue; one staging tile per team that has chunks (BN / 64 of them, at most 2)
   EpiArgs e;
 };
-
-__device__ __forceinline__ uint64_t sdesc_rows(uint32_t addr, int bo_mode) {
-  uint64_t d = make_sdesc_sw128(addr, 16, 1024);
-  if (bo_mode) d |= (uint64_t)((addr >> 7) & 7u) << 49;   // matrix base offset (start not on a 1024-byte boundary)
-  return d;
-}
 
 // One work item of a consumer warpgroup: both output rows' MMAs over every K block, accumulators for rows 0 / 1 in acc[0 / 1].
 template <int BN>
@@ -74,7 +68,7 @@ __device__ __forceinline__ void rows_mma_tile(const RowsArgs& p, float (&acc)[2]
       wgmma_fence();
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
-        const uint64_t adesc = sdesc_rows(sa + (kh + j) * kRowBufBytes + kw * 128, p.bo_mode);
+        const uint64_t adesc = make_sdesc_sw128(sa + (kh + j) * kRowBufBytes + kw * 128, 16, 1024);
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) Wgmma<BN>::template mma<0, 0>(acc[j], adesc + 2 * kk, bdesc + 2 * kk, 1u);
       }
@@ -239,42 +233,28 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 }
 
 void fill_epi(EpiArgs& e, const sgb_conv_desc* d);
-
-template <int F>
-static int launch_rows(int grid, size_t smem, cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmY,
-                       const RowsArgs& p) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    SGB_CUDA(cudaFuncSetAttribute(conv3x3_rows_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  conv3x3_rows_kernel<F><<<grid, kRowsThreads, smem, stream>>>(tmA, tmB, tmY, p);
-  SGB_LAUNCH_CHECK();
-  return SGB_OK;
-}
+int pick_bn(const sgb_conv_desc* d);
 
 bool conv3x3_rows_eligible(const sgb_conv_desc* d) {
   return d->KH == 3 && d->KW == 3 && d->pad_h == 1 && d->pad_w == 1 && d->w_mode == 0 && d->W % 128 == 0 && d->H % 2 == 0 &&
          d->Cin % 64 == 0 && d->Cin <= 128 && d->Cout % 8 == 0;
 }
 
-// bo_mode: 0 = no matrix base offset in the row-shifted descriptors (default), 1 = (addr >> 7) & 7.
-int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream, int bo_mode, int use_tma_env) {
+int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream) {
   RowsArgs p;
   p.B = d->B; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.Cout = d->Cout;
   p.kblocks = d->Cin / 64;
-  p.BN = d->Cout <= 16 ? 16 : d->Cout <= 32 ? 32 : d->Cout <= 64 ? 64 : 128;   // Cout = 8 (padded image channels) runs as one N = 16 tile
+  p.BN = pick_bn(d);      // Cout = 8 (padded image channels) runs as one N = 16 tile
   p.tiles_n = (d->Cout + p.BN - 1) / p.BN;
   p.segs = d->W / 128;
   p.hpairs = d->H / 2;
   p.num_tiles = p.tiles_n * p.segs * p.hpairs * d->B;
-  p.bo_mode = bo_mode;
   const uint32_t b_tile = p.BN * 128u;
   const uint32_t budget = 227u * 1024u - 2048u;
   const uint32_t a_stage = 4 * kRowBufBytes;
   const uint32_t resident_bytes = 9u * p.kblocks * b_tile;
   p.use_tma = (!d->y_fp32 && p.BN % 64 == 0 && d->y_cstride % 8 == 0 && (!d->residual || d->res_cstride % 8 == 0) &&
-               (!d->mask || d->mask_cstride % 8 == 0) && use_tma_env) ? 1 : 0;
+               (!d->mask || d->mask_cstride % 8 == 0)) ? 1 : 0;
   p.epi_bufs = p.BN >= 128 ? 2 : 1;
   const uint32_t fixed = 128u * rows_acc_ld(p.BN) + (p.use_tma ? p.epi_bufs * kEpiStageBytes : 0);
   p.resident = (p.tiles_n == 1 && resident_bytes + a_stage + fixed <= budget) ? 1 : 0;
@@ -292,26 +272,18 @@ int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream, int bo_mode
   fill_epi(p.e, d);
 
   CUtensorMap tmA, tmB;
-  {
-    uint64_t dims[4] = {(uint64_t)d->Cin, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->B};
-    uint64_t strides[3] = {(uint64_t)d->x_cstride * 2, (uint64_t)d->x_cstride * 2 * d->W, (uint64_t)d->x_cstride * 2 * d->W * d->H};
-    uint32_t box[4] = {64, (uint32_t)kRowPix, 1, 1};
-    int rc = make_tmap_bf16(&tmA, d->x, 4, dims, strides, box);
-    if (rc) return rc;
-  }
+  int rc = make_act_tmap(&tmA, d->x, d->B, d->H, d->W, d->Cin, d->x_cstride, kRowPix, 1, 1);
+  if (rc) return rc;
   {
     uint64_t dims[3] = {(uint64_t)d->Cin, 9, (uint64_t)d->Cout};
     uint64_t strides[2] = {(uint64_t)d->Cin * 2, (uint64_t)d->Cin * 2 * 9};
     uint32_t box[3] = {64, 1, (uint32_t)p.BN};
-    int rc = make_tmap_bf16(&tmB, d->w, 3, dims, strides, box);
+    rc = make_tmap_bf16(&tmB, d->w, 3, dims, strides, box);
     if (rc) return rc;
   }
   CUtensorMap tmY = tmA;
   if (p.use_tma) {
-    uint64_t dims[4] = {(uint64_t)d->Cout, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->B};
-    uint64_t strides[3] = {(uint64_t)d->y_cstride * 2, (uint64_t)d->y_cstride * 2 * d->W, (uint64_t)d->y_cstride * 2 * d->W * d->H};
-    uint32_t box[4] = {64, 128, 1, 1};
-    int rc = make_tmap_bf16(&tmY, d->y, 4, dims, strides, box);
+    rc = make_act_tmap(&tmY, d->y, d->B, d->H, d->W, d->Cout, d->y_cstride, 128, 1, 1);
     if (rc) return rc;
   }
   const int nb = p.resident ? 1 : p.b_stages;
@@ -321,17 +293,18 @@ int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream, int bo_mode
   SGB_REQUIRE(smem <= 227u * 1024u);
   const int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
   const int f = p.use_tma ? epi_flags_of(p.e) : -1;
+#define SGB_ROWS_CASE(FLAGS) \
+  case (FLAGS): return launch_kernel<conv3x3_rows_kernel<(FLAGS)>>(grid, kRowsThreads, smem, stream, tmA, tmB, tmY, p);
   switch (f) {
-    case kEpiFull | kEpiBias: return launch_rows<kEpiFull | kEpiBias>(grid, smem, stream, tmA, tmB, tmY, p);                        // generator 3x3
-    case kEpiFull | kEpiBias | kEpiRelu: return launch_rows<kEpiFull | kEpiBias | kEpiRelu>(grid, smem, stream, tmA, tmB, tmY, p);    // discriminator 3x3
-    case kEpiFull | kEpiBias | kEpiRelu | kEpiBitsOut:
-      return launch_rows<kEpiFull | kEpiBias | kEpiRelu | kEpiBitsOut>(grid, smem, stream, tmA, tmB, tmY, p);                         // ... writing the ReLU bit plane
-    case kEpiFull | kEpiMask: return launch_rows<kEpiFull | kEpiMask>(grid, smem, stream, tmA, tmB, tmY, p);                        // dgrad through a ReLU (bf16 mask)
-    case kEpiFull | kEpiMask | kEpiMaskBits:
-      return launch_rows<kEpiFull | kEpiMask | kEpiMaskBits>(grid, smem, stream, tmA, tmB, tmY, p);                                   // dgrad through a ReLU (bit plane)
-    case kEpiFull: return launch_rows<kEpiFull>(grid, smem, stream, tmA, tmB, tmY, p);                                              // plain dgrad
-    default: return launch_rows<-1>(grid, smem, stream, tmA, tmB, tmY, p);
+    SGB_ROWS_CASE(kEpiFull | kEpiBias)                                  // generator 3x3
+    SGB_ROWS_CASE(kEpiFull | kEpiBias | kEpiRelu)                       // discriminator 3x3
+    SGB_ROWS_CASE(kEpiFull | kEpiBias | kEpiRelu | kEpiBitsOut)         // ... writing the ReLU bit plane
+    SGB_ROWS_CASE(kEpiFull | kEpiMask)                                  // dgrad through a ReLU (bf16 mask)
+    SGB_ROWS_CASE(kEpiFull | kEpiMask | kEpiMaskBits)                   // dgrad through a ReLU (bit plane)
+    SGB_ROWS_CASE(kEpiFull)                                             // plain dgrad
+    default: return launch_kernel<conv3x3_rows_kernel<-1>>(grid, kRowsThreads, smem, stream, tmA, tmB, tmY, p);
   }
+#undef SGB_ROWS_CASE
 }
 
 }  // namespace sgb

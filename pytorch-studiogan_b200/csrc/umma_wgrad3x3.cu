@@ -178,19 +178,9 @@ int launch_wgrad3x3_c64(const sgb_wgrad_desc* d, cudaStream_t stream) {
     if (d->dbias) SGB_CUDA(cudaMemsetAsync(d->dbias, 0, sizeof(float) * (size_t)d->Cout, stream));
   }
   CUtensorMap tmDY;
-  {
-    uint64_t dims[4] = {(uint64_t)d->Cout, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->B};
-    uint64_t strides[3] = {(uint64_t)d->dy_cstride * 2, (uint64_t)d->dy_cstride * 2 * d->W, (uint64_t)d->dy_cstride * 2 * d->W * d->H};
-    uint32_t box[4] = {64, (uint32_t)kW3Px, 2, 1};
-    int rc = make_tmap_bf16(&tmDY, d->dy, 4, dims, strides, box);
-    if (rc) return rc;
-  }
+  int rc = make_act_tmap(&tmDY, d->dy, d->B, d->H, d->W, d->Cout, d->dy_cstride, kW3Px, 2, 1);
+  if (rc) return rc;
   const size_t smem = (size_t)kW3Stages * kW3Stage + 1024 + 1024 + 8 * (2 * kW3Stages);
-  static bool attr_set = false;
-  if (!attr_set) {
-    SGB_CUDA(cudaFuncSetAttribute(wgrad3x3_c64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
   for (int ci0 = 0; ci0 < d->Cin; ci0 += 64) {
     W3Args p;
     p.H = d->H; p.W = d->W; p.Cout = d->Cout;
@@ -202,14 +192,11 @@ int launch_wgrad3x3_c64(const sgb_wgrad_desc* d, cudaStream_t stream) {
     p.dw = d->dw + ci0;
     p.dbias = ci0 == 0 ? d->dbias : nullptr;
     CUtensorMap tmX;
-    uint64_t dims[4] = {(uint64_t)p.Cin, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->B};
-    uint64_t strides[3] = {(uint64_t)d->x_cstride * 2, (uint64_t)d->x_cstride * 2 * d->W, (uint64_t)d->x_cstride * 2 * d->W * d->H};
-    uint32_t box[4] = {64, (uint32_t)kW3Halo, 4, 1};
-    int rc = make_tmap_bf16(&tmX, (const bf16*)d->x + ci0, 4, dims, strides, box);
+    rc = make_act_tmap(&tmX, (const bf16*)d->x + ci0, d->B, d->H, d->W, p.Cin, d->x_cstride, kW3Halo, 4, 1);
     if (rc) return rc;
     const int grid = p.tiles < sm_count() ? (int)p.tiles : sm_count();
-    wgrad3x3_c64_kernel<<<grid, kW3Threads, smem, stream>>>(tmDY, tmX, p);
-    SGB_LAUNCH_CHECK();
+    rc = launch_kernel<wgrad3x3_c64_kernel>(grid, kW3Threads, smem, stream, tmDY, tmX, p);
+    if (rc) return rc;
   }
   return SGB_OK;
 }

@@ -4,8 +4,6 @@ ConditionalBatchNorm2d / SelfAttention / init_weights), but every forward runs l
 activations.  Modules subclass nn.Conv2d / nn.Linear / nn.Embedding / nn.BatchNorm2d so that the reference's
 ``isinstance`` based toggles (src/utils/misc.py:192-267,345-364) keep matching.
 """
-import os
-
 import numpy as np
 import torch
 import torch.nn as nn
@@ -321,7 +319,8 @@ def quantize_images(x):
 # one embedding row product per image) is a few kFLOP and is expressed directly on those tensors.  Spectral norm of the
 # head layers still goes through the library's power-iteration kernel so u / v evolve exactly like every other layer.
 # ----------------------------------------------------------------------------------------------------------------------
-DHEAD_FUSED = os.environ.get("SGB_DHEAD", "1") != "0"     # A/B switch: 0 = the head as eager tensor arithmetic
+_HEAD_KEYS = ["embed", "proxy", "cls_output", "mi_embed", "mi_proxy", "mi_cls_output", "info_discrete_c_logits", "info_conti_mu",
+              "info_conti_var"]
 
 
 def _head_weight(module):
@@ -363,18 +362,24 @@ def discriminator_head(D, h, label, adc_fake=False):
     """Everything after ``h = sum(relu(features), [2, 3])`` in the reference discriminators
     (src/models/big_resnet_deep_legacy.py:347-413; identical in big_resnet.py / resnet.py): adversarial logit,
     class conditioning (PD / AC / 2C / D2DCE / MD / MH), TAC / ADC extras, and the 12-key result dict."""
-    out = dict.fromkeys(["embed", "proxy", "cls_output", "mi_embed", "mi_proxy", "mi_cls_output",
-                         "info_discrete_c_logits", "info_conti_mu", "info_conti_var"])
     mtd = D.d_cond_mtd
-    if (DHEAD_FUSED and mtd in ("PD", "W/O") and D.aux_cls_type in ("W/O", "N/A", None) and D.linear1.out_features == 1 and h.is_cuda
+    if not (mtd in ("PD", "W/O") and D.aux_cls_type in ("W/O", "N/A", None) and D.linear1.out_features == 1 and h.is_cuda
             and h.dtype == torch.float32 and h.shape[1] % 8 == 0):
-        # hot-path heads (projection discriminator / unconditional): one library launch forward, two backward (A.DHeadFn)
-        E = D.embedding if mtd == "PD" else None
-        cfg = {"sn1": getattr(D.linear1, "_sn", None), "snE": getattr(E, "_sn", None) if E is not None else None,
-               "training": D.linear1.training}
-        adv = A.DHeadFn.call(h, _w(D.linear1), D.linear1.bias, _w(E) if E is not None else None, label, cfg)
-        out.update({"h": h, "adv_output": adv, "label": label})
-        return out
+        return _head_tensor_ops(D, h, label, adc_fake)
+    # hot-path heads (projection discriminator / unconditional): one library launch forward, two backward (A.DHeadFn)
+    E = D.embedding if mtd == "PD" else None
+    cfg = {"sn1": getattr(D.linear1, "_sn", None), "snE": getattr(E, "_sn", None) if E is not None else None,
+           "training": D.linear1.training}
+    adv = A.DHeadFn.call(h, _w(D.linear1), D.linear1.bias, _w(E) if E is not None else None, label, cfg)
+    out = dict.fromkeys(_HEAD_KEYS)
+    out.update({"h": h, "adv_output": adv, "label": label})
+    return out
+
+
+def _head_tensor_ops(D, h, label, adc_fake):
+    """discriminator_head written as tensor arithmetic on h: every head that sgb_dhead_fwd / bwd do not cover."""
+    out = dict.fromkeys(_HEAD_KEYS)
+    mtd = D.d_cond_mtd
     w_eff = _head_weight(D.linear1)
     adv = torch.squeeze(F.linear(h, w_eff, D.linear1.bias))
     if D.aux_cls_type == "ADC":

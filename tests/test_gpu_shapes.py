@@ -64,6 +64,109 @@ def test_per_image_wgrad_at_attention_size():
     assert rel_err(got.view(B, M, c8), ref) < 2e-3
 
 
+# ------------------------------------------------------------------------------------------------ conv engine case table
+# id: (B, H, W, Cin, Cout, KH, KW, bias, relu, residual, res_up2, bf16 mask, fp32 output).  Generic kernel: K blocks, ragged
+# and batched pixel tiles, Cin / Cout not multiples of 64; halo-row kernel ("rows"): resident / ring filters, every output
+# tile 16..128, fp32 output, bf16 mask, up-sampled residual; "aux": residual / mask tiles through the epilogue's TMA ring.
+FPROP_CASES = {
+    "1x1 c64-64 16x16":             (2, 16, 16, 64, 64, 1, 1, 0, 0, 0, 0, 0, 1),
+    "1x1 c128-128 16x16":           (2, 16, 16, 128, 128, 1, 1, 0, 0, 0, 0, 0, 1),
+    "1x1 c256-64 8x8 bias":         (4, 8, 8, 256, 64, 1, 1, 1, 0, 0, 0, 0, 0),
+    "3x3 c64-64 8x8":               (2, 8, 8, 64, 64, 3, 3, 0, 0, 0, 0, 0, 1),
+    "3x3 c128-256 32x32 b/r/res":   (2, 32, 32, 128, 256, 3, 3, 1, 1, 1, 0, 0, 0),
+    "3x3 c64-3 16x16 bias":         (2, 16, 16, 64, 3, 3, 3, 1, 0, 0, 0, 0, 1),
+    "3x3 c8-64 16x16":              (2, 16, 16, 8, 64, 3, 3, 1, 0, 0, 0, 0, 0),
+    "linear 256-512 B=256":         (256, 1, 1, 256, 512, 1, 1, 1, 0, 0, 0, 0, 1),
+    "3x3 4x4 ragged B=12":          (12, 4, 4, 64, 128, 3, 3, 1, 0, 0, 0, 0, 0),
+    "1x1 res_up2+mask 16x16":       (2, 16, 16, 64, 64, 1, 1, 1, 1, 1, 1, 1, 0),
+    "1x7 c64-96 17x17 ragged":      (2, 17, 17, 64, 96, 1, 7, 1, 1, 0, 0, 0, 0),
+    "3x3 c192-320 64x64":           (1, 64, 64, 192, 320, 3, 3, 1, 0, 0, 0, 0, 0),
+    "3x3 c64-64 256x256":           (1, 256, 256, 64, 64, 3, 3, 0, 0, 0, 0, 0, 0),
+    "rows c64-64 b/r/res":          (2, 128, 128, 64, 64, 3, 3, 1, 1, 1, 0, 0, 0),
+    "rows c128-128 mask":           (1, 128, 128, 128, 128, 3, 3, 1, 0, 0, 0, 1, 0),
+    "rows c64-128 up2res":          (1, 128, 128, 64, 128, 3, 3, 1, 0, 1, 1, 0, 0),
+    "rows c128-64 256x256 fp32":    (1, 256, 256, 128, 64, 3, 3, 0, 0, 0, 0, 0, 1),
+    "rows c64-192":                 (1, 128, 128, 64, 192, 3, 3, 1, 0, 0, 0, 0, 0),
+    "rows c64-16":                  (3, 128, 128, 64, 16, 3, 3, 1, 0, 0, 0, 0, 0),
+    "rows c128-8":                  (2, 128, 128, 128, 8, 3, 3, 1, 0, 0, 0, 0, 0),
+    "aux 1x1 c64-256 32x32 res":    (2, 32, 32, 64, 256, 1, 1, 1, 0, 1, 0, 0, 0),
+    "aux 1x1 c64-128 32x32 up2res": (2, 32, 32, 64, 128, 1, 1, 1, 0, 1, 1, 0, 0),
+    "aux 1x1 c128-64 16x16 mask":   (3, 16, 16, 128, 64, 1, 1, 0, 0, 0, 0, 1, 0),
+    "aux 3x3 c64-64 res+relu":      (2, 16, 16, 64, 64, 3, 3, 1, 1, 1, 0, 0, 0),
+    "aux 1x1 c64-256 4x4 up2 B=12": (12, 4, 4, 64, 256, 1, 1, 1, 0, 1, 1, 0, 0),
+    "aux 1x1 c64-192 8x8 res":      (5, 8, 8, 64, 192, 1, 1, 1, 0, 1, 0, 0, 0),
+    "aux 1x1 c64-128 256x128 up2":  (1, 256, 128, 64, 128, 1, 1, 0, 0, 1, 1, 0, 0),
+    "aux 1x1 c32-64 64x64 mask":    (2, 64, 64, 32, 64, 1, 1, 1, 0, 0, 0, 1, 0),
+}
+
+
+@pytest.mark.parametrize("B,H,W,Cin,Cout,KH,KW,bias,relu,res,up2,mask,fp32", list(FPROP_CASES.values()), ids=list(FPROP_CASES))
+def test_conv_fprop_epilogue_cases(B, H, W, Cin, Cout, KH, KW, bias, relu, res, up2, mask, fp32):
+    """y = mask(relu(0.5 * conv(x, w) + bias + residual)) against fp32 torch on the CPU with the same bf16 operands."""
+    from sgb200 import kernels as K
+    dev = _cuda()
+    g = torch.Generator().manual_seed(B * 1000 + H + Cin * 7 + Cout + KW)
+    x = bfr(torch.rand(B, Cin, H, W, generator=g) - 0.5)
+    w = bfr((torch.rand(Cout, Cin, KH, KW, generator=g) - 0.5) * 0.25)
+    b = torch.rand(Cout, generator=g) - 0.5
+    r = bfr(torch.rand(B, Cout, H // 2 if up2 else H, W // 2 if up2 else W, generator=g) - 0.5)
+    m = bfr(torch.rand(B, Cout, H, W, generator=g) - 0.5)
+    ref = 0.5 * F.conv2d(x, w, padding=(KH // 2, KW // 2))
+    if bias:
+        ref = ref + b.view(1, -1, 1, 1)
+    if res:
+        ref = ref + (r.repeat_interleave(2, 2).repeat_interleave(2, 3) if up2 else r)
+    if relu:
+        ref = ref.clamp_min(0)
+    if mask:
+        ref = torch.where(m > 0, ref, torch.zeros(()))
+    wf, _ = K.weight_pack(w.to(dev), None, Cout, Cin, KH * KW, True, False)
+    y = K.conv_fprop(to_nhwc(x, dev), wf, Cout, KH, KW, KH // 2, KW // 2, bias=b.to(dev) if bias else None,
+                     residual=to_nhwc(r, dev) if res else None, res_up2=bool(up2), mask=to_nhwc(m, dev) if mask else None,
+                     relu=bool(relu), alpha=0.5, out_fp32=bool(fp32))
+    assert y.dtype == (torch.float32 if fp32 else torch.bfloat16)
+    assert rel_err(y, ref) < 8e-3
+
+
+# id: (B, H, W, Cin, Cout, KH, KW).  "w3": the 64-channel 3x3 weight-gradient kernel (Cin 32 / 64, one launch per 64-channel
+# block at Cin 128); the rest take the generic kernel.
+WGRAD_CASES = {
+    "1x1 c64-64 16x16":        (2, 16, 16, 64, 64, 1, 1),
+    "1x1 c128-128 16x16":      (2, 16, 16, 128, 128, 1, 1),
+    "1x1 c256-64 8x8":         (4, 8, 8, 256, 64, 1, 1),
+    "3x3 c64-64 8x8":          (2, 8, 8, 64, 64, 3, 3),
+    "3x3 c128-256 32x32":      (2, 32, 32, 128, 256, 3, 3),
+    "3x3 c64-8 16x16":         (2, 16, 16, 64, 8, 3, 3),
+    "3x3 c8-64 16x16":         (2, 16, 16, 8, 64, 3, 3),
+    "linear 256-512 B=256":    (256, 1, 1, 256, 512, 1, 1),
+    "3x3 4x4 ragged B=12":     (12, 4, 4, 64, 128, 3, 3),
+    "1x7 c64-96 17x17 ragged": (2, 17, 17, 64, 96, 1, 7),
+    "3x3 c192-320 64x64":      (1, 64, 64, 192, 320, 3, 3),
+    "w3 c64-64 128x128 B=2":   (2, 128, 128, 64, 64, 3, 3),
+    "w3 c64-64 8x256 B=3":     (3, 8, 256, 64, 64, 3, 3),
+    "w3 c64-32 128x128":       (1, 128, 128, 64, 32, 3, 3),
+    "w3 c32-64 128x128":       (1, 128, 128, 32, 64, 3, 3),
+    "w3 c64-64 128x128 B=5":   (5, 128, 128, 64, 64, 3, 3),
+    "w3 c128-8 128x128":       (2, 128, 128, 128, 8, 3, 3),
+}
+
+
+@pytest.mark.parametrize("B,H,W,Cin,Cout,KH,KW", list(WGRAD_CASES.values()), ids=list(WGRAD_CASES))
+def test_conv_wgrad_cases(B, H, W, Cin, Cout, KH, KW):
+    """Weight gradient in the fprop-pack layout [Cout][KH*KW][Cin], and the bias gradient where the launch fuses it, against
+    fp32 torch on the CPU with the same bf16 operands."""
+    from sgb200 import kernels as K
+    dev = _cuda()
+    g = torch.Generator().manual_seed(B * 1000 + H + Cin * 7 + Cout + KW)
+    x = bfr(torch.rand(B, Cin, H, W, generator=g) - 0.5)
+    dy = bfr(torch.rand(B, Cout, H, W, generator=g) - 0.5)
+    ref = torch.nn.grad.conv2d_weight(x, (Cout, Cin, KH, KW), dy, padding=(KH // 2, KW // 2))
+    dw, db = K.conv_wgrad(to_nhwc(x, dev), to_nhwc(dy, dev), KH, KW, KH // 2, KW // 2, want_dbias=True)
+    assert rel_err(dw, ref.permute(0, 2, 3, 1).reshape(Cout, KH * KW, Cin)) < 2e-3
+    if db is not None:
+        assert rel_err(db, dy.sum((0, 2, 3))) < 2e-3
+
+
 # ------------------------------------------------------------------------------------------------ full model at 256x256
 def _digest_errors(net, g, prefix):
     """Checks a gradient against tests/golden/make_golden.py::grad_digest: full tensors where stored, else norm + seeded
@@ -436,7 +539,7 @@ def test_relu_bit_planes_written_and_consumed(B, H, W, Cin, Cout, k):
         assert diff.any() or torch.equal(a, c)
 
 
-def test_pool2_bwd_with_bit_planes_and_d_block_uses_them():
+def test_pool2_bwd_with_bit_planes_and_d_block_always_uses_them():
     from sgb200 import kernels as K
     dev = _cuda()
     g = torch.Generator().manual_seed(3)
@@ -461,8 +564,7 @@ def test_pool2_bwd_with_bit_planes_and_d_block_uses_them():
     lab = torch.randint(0, 5, (4,), generator=g).to(dev)
     K.BITS_STATS.update(written=0, used=0)
     D(img, lab)["adv_output"].sum().backward()
-    if K.RELU_BITS:
-        assert K.BITS_STATS["written"] > 0 and K.BITS_STATS["used"] >= K.BITS_STATS["written"] - 1, K.BITS_STATS   # (the head reads the last tensor itself)
+    assert K.BITS_STATS["written"] > 0 and K.BITS_STATS["used"] >= K.BITS_STATS["written"] - 1, K.BITS_STATS   # (the head reads the last tensor itself)
 
 
 @pytest.mark.parametrize("B,S,c8,c2", [(2, 64, 64, 256), (3, 16, 48, 192), (1, 32, 16, 64)])
@@ -527,14 +629,10 @@ def test_discriminator_head_kernels_match_the_eager_head(mtd, sn):
     h0 = (torch.rand(6, C, generator=g) * 3).to(dev)
     lab = torch.randint(0, 7, (6,), generator=g).to(dev)
     res = []
-    for D, fused in ((D1, True), (D2, False)):
-        ops.DHEAD_FUSED = fused
-        try:
-            h = h0.clone().requires_grad_(True)
-            adv = ops.discriminator_head(D, h, lab)["adv_output"]
-            (adv * torch.arange(1, 7, device=dev).float()).sum().backward()
-        finally:
-            ops.DHEAD_FUSED = True
+    for D, head in ((D1, ops.discriminator_head), (D2, ops._head_tensor_ops)):
+        h = h0.clone().requires_grad_(True)
+        adv = head(D, h, lab, False)["adv_output"]
+        (adv * torch.arange(1, 7, device=dev).float()).sum().backward()
         pg = {n: p.grad.clone() for n, p in D.named_parameters() if p.grad is not None}
         res.append((adv.detach(), h.grad.clone(), pg))
     (a1, dh1, g1), (a2, dh2, g2) = res
