@@ -459,4 +459,113 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
   }
 }
 
+// -------------------------------------------------------------------------------------------------------------------
+// Epilogue straight from the wgmma accumulator registers of one warpgroup: 64 pixel rows x BN channels in the Wgmma
+// fragment layout (thread = warp w, lane l of the warpgroup: rows 16w + l/4 and 16w + l/4 + 8, columns 8j + 2(l%4) + 0 / 1).
+// No fp32 staging: per 64-channel chunk the warpgroup packs bf16 pairs into a SWIZZLE_128B staging tile [64 rows][64 ch]
+// (8 KiB; a thread's pair of column block j goes to 16-byte unit j ^ (row & 7), conflict-free) and one thread issues the
+// TMA store of the box (64 ch, 64 px).  Per element the arithmetic is that of epilogue_tile_tma's piece(): acc * alpha,
+// + bias, fmaf(residual, rs, .), ReLU, mask, fmaf(post-mask residual, rs, .), bf16 pack -- the outputs are bit-identical.
+// ReLU bit planes are OR-reduced over the four lanes that share a row.  Residual and bf16 mask are read from global memory.
+//   pix / rpix : output / residual pixel of this thread's two rows.  stage: this warpgroup's first staging tile (1024-aligned),
+//   nbuf tiles used round-robin (sbuf = next one).  bar: named barrier of the warpgroup.
+template <int F, int BN>
+__device__ __forceinline__ void epilogue_frag_tma(const EpiArgs& p, const CUtensorMap* tmY, const float (&acc)[BN / 2], int n0,
+                                                  int c1, int c2, int c3, const long long (&pix)[2], const long long (&rpix)[2],
+                                                  float alpha, uint32_t stage, int nbuf, uint32_t& sbuf, uint32_t bar, bool leader) {
+  static_assert(F < 0 || (F & (kEpiSmStats | kEpiSmApply | kEpiSmBwd | kEpiAuxRes | kEpiAuxMask)) == 0,
+                "softmax and aux-ring epilogues are served by epilogue_tile_tma");
+  constexpr uint32_t kFragStageBytes = 64 * 128;
+  const bool has_bias = F < 0 ? p.bias != nullptr : (F & kEpiBias) != 0;
+  const bool do_relu = F < 0 ? p.relu != 0 : (F & kEpiRelu) != 0;
+  const bool res_pre = F < 0 ? (p.residual != nullptr && !p.res_after) : (F & kEpiResPre) != 0;
+  const bool res_post = F < 0 ? (p.residual != nullptr && p.res_after) : (F & kEpiResPost) != 0;
+  const bool has_mask = F < 0 ? (p.mask != nullptr || p.mask_bits != nullptr) : (F & kEpiMask) != 0;
+  const bool use_mbits = F < 0 ? (has_mask && p.mask_bits != nullptr) : (F & kEpiMaskBits) != 0;
+  const bool emit_bits = F < 0 ? (do_relu && p.relu_bits != nullptr) : (F & kEpiBitsOut) != 0;
+  constexpr bool bits_from_packed = F >= 0 && (F & kEpiBitsOut) != 0 && (F & (kEpiMask | kEpiResPost)) == 0;
+  const bool full_c = F >= 0 && (F & kEpiFull) != 0;
+  const float rs = p.res_scale;
+  const long long nw = p.Cout >> 6;
+  const uint32_t w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31, q = l & 3;
+  const uint32_t r0 = 16u * w + (l >> 2);
+#pragma unroll                                   // static accumulator indices: the fragments stay in registers
+  for (int cc = 0; cc * 64 < BN; ++cc) {
+    const int nbase = n0 + cc * 64;
+    if (!full_c && nbase >= p.Cout) break;
+    const uint32_t stage_cur = stage + sbuf * kFragStageBytes;
+    if (leader) {                                // the store that last used this staging tile has finished reading it
+      if (nbuf == 1) bulk_wait_read0();
+      else bulk_wait_read1();
+    }
+    sbuf = (sbuf + 1u == (uint32_t)nbuf) ? 0u : sbuf + 1u;
+    named_bar_sync(bar, 128);
+    uint32_t mb[2][2] = {{0u, 0u}, {0u, 0u}}, ob[2][2] = {{0u, 0u}, {0u, 0u}};
+    if (use_mbits) {
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const uint2 m = __ldg(reinterpret_cast<const uint2*>(p.mask_bits) + pix[hr] * nw + (nbase >> 6));
+        mb[hr][0] = m.x; mb[hr][1] = m.y;
+      }
+    }
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int j = cc * 8 + jj;                 // 8-column block of the accumulator
+      const int n = nbase + 8 * jj + 2 * (int)q;
+      const bool in_c = full_c || nbase + 8 * jj < p.Cout;      // Cout % 8 == 0: a column block is all in or all out
+      const uint32_t bit = 8u * (jj & 3) + 2u * q;              // bit of column 0 of the pair in its 32-bit half of the word
+      float2 bb = make_float2(0.f, 0.f);
+      if (has_bias && in_c) bb = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        float f0 = acc[4 * j + 2 * hr] * alpha, f1 = acc[4 * j + 2 * hr + 1] * alpha;
+        if (has_bias && in_c) { f0 += bb.x; f1 += bb.y; }
+        if (res_pre && in_c) {
+          const uint32_t r = __ldg(reinterpret_cast<const unsigned int*>(p.residual + rpix[hr] * p.res_cstride + n));
+          f0 = fmaf(bf16_bits_lo(r), rs, f0); f1 = fmaf(bf16_bits_hi(r), rs, f1);
+        }
+        if (do_relu) {
+          f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f);
+          if (emit_bits && !bits_from_packed) ob[hr][jj >> 2] |= ((f0 > 0.f) ? 1u : 0u) << bit | ((f1 > 0.f) ? 1u : 0u) << (bit + 1);
+        }
+        if (use_mbits) {
+          const uint32_t m = mb[hr][jj >> 2] >> bit;
+          f0 = (m & 1u) ? f0 : 0.f; f1 = (m & 2u) ? f1 : 0.f;
+        } else if (has_mask && in_c) {
+          const uint32_t m = __ldg(reinterpret_cast<const unsigned int*>(p.mask + pix[hr] * p.mask_cstride + n));
+          f0 = bf16_bits_lo(m) > 0.f ? f0 : 0.f; f1 = bf16_bits_hi(m) > 0.f ? f1 : 0.f;
+        }
+        if (res_post && in_c) {
+          const uint32_t r = __ldg(reinterpret_cast<const unsigned int*>(p.residual + rpix[hr] * p.res_cstride + n));
+          f0 = fmaf(bf16_bits_lo(r), rs, f0); f1 = fmaf(bf16_bits_hi(r), rs, f1);
+        }
+        const uint32_t pk = pack_bf16x2(f0, f1);
+        if (bits_from_packed) {                  // as positive_bits16_packed: a half is flagged iff it is not +0
+          const uint32_t t = pk + 0x7FFF7FFFu;
+          ob[hr][jj >> 2] |= ((t >> 15) & 1u) << bit | (t >> 31) << (bit + 1);
+        }
+        const uint32_t r = r0 + 8u * hr;
+        st_shared_b32(stage_cur + r * 128u + ((((uint32_t)jj) ^ (r & 7u)) << 4) + 4u * q, pk);
+      }
+    }
+    if (emit_bits) {
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          ob[hr][k] |= __shfl_xor_sync(0xffffffffu, ob[hr][k], 1);
+          ob[hr][k] |= __shfl_xor_sync(0xffffffffu, ob[hr][k], 2);
+        }
+        if (q == 0) reinterpret_cast<uint2*>(p.relu_bits)[pix[hr] * nw + (nbase >> 6)] = make_uint2(ob[hr][0], ob[hr][1]);
+      }
+    }
+    fence_proxy_async_smem();                    // generic-proxy smem writes -> visible to the TMA (async proxy)
+    named_bar_sync(bar, 128);
+    if (leader) {
+      tma_store_4d(tmY, stage_cur, nbase, c1, c2, c3);
+      bulk_commit();
+    }
+  }
+}
+
 }  // namespace sgb

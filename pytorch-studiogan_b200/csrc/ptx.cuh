@@ -93,6 +93,19 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t a) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory");
+}
+
+// ---------------------------------------------------------------- register reallocation between warpgroups
+// Executed by all 128 threads of a warpgroup.  A 384-thread CTA launched at 168 registers per thread (the
+// __launch_bounds__(384, 1) cap) can move 128 x (168 - 40) registers from the producer warpgroup to the two consumer
+// warpgroups: 128 x 40 + 256 x 232 = 64 512 <= 65 536.
+template <int R>
+__device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+static constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 
 // ---------------------------------------------------------------- wgmma
 // D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 inputs from shared-memory descriptors, f32 accumulators in registers; issued by

@@ -9,8 +9,11 @@
 //                 function of the absolute shared-memory address, so a row-shifted descriptor addresses exactly what TMA wrote
 //   B staging   = filter taps; RESIDENT in smem for the whole persistent CTA when they fit (C = 64: 72 KiB), else a ring
 //   L2 traffic  = 33 KiB per 128 output pixels at C = 64 (was 216 KiB), 210 KiB at C = 128 (was 576 KiB)
-// Warps: 0 = A producer, 2 = B producer; warpgroups 1 and 2 = consumers (pixels 0..63 / 64..127 of the row, wgmma M = 64),
-// which stage each output row's accumulators in shared memory and run the fused epilogue on it.
+// Warps: 0 = A producer, 2 = B producer (warpgroup 0 gives up registers with setmaxnreg); warpgroups 1 and 2 = consumers
+// (pixels 0..63 / 64..127 of the row, wgmma M = 64).  Each consumer warpgroup runs the fused epilogue straight from its
+// accumulator registers and TMA-stores its 64 pixels through its own bf16 staging tiles (epilogue_frag_tma), so no fp32
+// staging competes with the halo ring: both hot shapes (C = 64 resident taps, C = 128 filter ring) get two halo stages, and the
+// next item's halo rows load while this item computes.  fp32 outputs, N < 64 and unaligned strides take the staged-row epilogue.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "conv_epilogue.cuh"
@@ -30,9 +33,15 @@ struct RowsArgs {
   int B, H, W, Cin, Cout;
   int kblocks, BN, tiles_n, segs, hpairs, num_tiles;
   int resident, a_stages, b_stages;
-  int use_tma, epi_bufs;   // TMA-store epilogue; one staging tile per team that has chunks (BN / 64 of them, at most 2)
+  int use_tma, epi_nbuf;   // fragment epilogue with TMA stores; 8 KiB bf16 staging tiles per consumer warpgroup
   EpiArgs e;
 };
+
+// Shared memory in front of the operand rings: the bf16 staging tiles of the fragment epilogue, or (staged-row epilogue) the
+// fp32 accumulator rows of one output row.  A multiple of 1024 bytes.
+__host__ __device__ inline uint32_t rows_epi_bytes(const RowsArgs& p) {
+  return p.use_tma ? 2u * (uint32_t)p.epi_nbuf * 64u * 128u : 128u * rows_acc_ld(p.BN);
+}
 
 // One work item of a consumer warpgroup: both output rows' MMAs over every K block, accumulators for rows 0 / 1 in acc[0 / 1].
 template <int BN>
@@ -99,47 +108,74 @@ __device__ __forceinline__ void rows_stage(const float (&acc)[BN / 2], uint32_t 
 }
 
 template <int F, int BN>
-__device__ __forceinline__ void rows_consumer(const RowsArgs& p, const CUtensorMap* tmY, uint32_t epi_stage_base, uint32_t acc_base,
-                                              uint32_t a_base, uint32_t a_stage_bytes, uint32_t b_base, uint32_t b_tile_bytes,
-                                              uint32_t bar_base, int nb) {
+__device__ __forceinline__ void rows_consumer(const RowsArgs& p, const CUtensorMap* tmY, uint32_t epi_base, uint32_t a_base,
+                                              uint32_t a_stage_bytes, uint32_t b_base, uint32_t b_tile_bytes, uint32_t bar_base, int nb) {
   const int ct = threadIdx.x - 128;
-  const int wg = ct >> 7, team = wg;
+  const int wg = ct >> 7;
   const int q = (ct >> 5) & 3;
   const int lane = threadIdx.x & 31;
-  const int row = q * 32 + lane;
-  const bool leader = (q == 0) && (lane == 0);
-  const bool vec_ok = epi_vec_ok(p.e);
   const float alpha = p.e.alpha_ptr ? p.e.alpha * __ldg(p.e.alpha_ptr) : p.e.alpha;
-  const uint32_t t_row = acc_base + (uint32_t)row * rows_acc_ld(BN);
   uint32_t ita = 0, itb = 0;
   if (p.resident) mbar_wait(bar_base + 8u * (2 * p.a_stages), 0);
-  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-    int t = tile;
-    const int nt = t % p.tiles_n; t /= p.tiles_n;
-    const int ws = t % p.segs; t /= p.segs;
-    const int hp = t % p.hpairs; t /= p.hpairs;
-    const int b = t;
-    float acc[2][BN / 2];
-    rows_mma_tile<BN>(p, acc, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb, ita, itb, wg);
-    const int w = ws * 128 + row;
+  if constexpr (F < 0 || BN < 64) {
+    if (!p.use_tma) {
+      // staged-row epilogue (fp32 output, N < 64, unaligned strides): both rows' accumulators go through shared memory and
+      // warpgroup 1 runs epilogue_row, one thread per pixel
+      const int row = q * 32 + lane;
+      const bool vec_ok = epi_vec_ok(p.e);
+      const uint32_t t_row = epi_base + (uint32_t)row * rows_acc_ld(BN);
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        int t = tile;
+        const int nt = t % p.tiles_n; t /= p.tiles_n;
+        const int ws = t % p.segs; t /= p.segs;
+        const int hp = t % p.hpairs; t /= p.hpairs;
+        const int b = t;
+        float acc[2][BN / 2];
+        rows_mma_tile<BN>(p, acc, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb, ita, itb, wg);
+        const int w = ws * 128 + row;
 #pragma unroll 1
-    for (int j = 0; j < 2; ++j) {
-      if (j == 0) rows_stage<BN>(acc[0], acc_base, wg);    // static indices keep both accumulators in registers
-      else rows_stage<BN>(acc[1], acc_base, wg);
-      const int h = hp * 2 + j;
-      const long long pix = ((long long)b * p.H + h) * p.W + w;
-      const long long rpix = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1)) : pix;
-      if (p.use_tma) {
-        // the two teams take alternate 64-channel chunks of the row, each through its own staging tile
-        if (team < p.epi_bufs)
-          epilogue_tile_tma<F>(p.e, tmY, t_row, BN, nt * BN, ws * 128, h, b, true, pix, rpix, alpha, epi_stage_base + team * kEpiStageBytes,
-                               team, row, leader, 2);
-      } else if (team == 0) {
-        epilogue_row(p.e, t_row, BN, nt * BN, true, pix, rpix, alpha, vec_ok);
+        for (int j = 0; j < 2; ++j) {
+          if (j == 0) rows_stage<BN>(acc[0], epi_base, wg);    // static indices keep both accumulators in registers
+          else rows_stage<BN>(acc[1], epi_base, wg);
+          const int h = hp * 2 + j;
+          const long long pix = ((long long)b * p.H + h) * p.W + w;
+          const long long rpix = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1)) : pix;
+          if (wg == 0) epilogue_row(p.e, t_row, BN, nt * BN, true, pix, rpix, alpha, vec_ok);
+        }
       }
+      return;
     }
   }
-  if (p.use_tma && leader && team < p.epi_bufs) bulk_wait_all();
+  if constexpr (BN >= 64) {
+    // fragment epilogue: each warpgroup stores its 64 pixels of both rows from its registers through its own staging tiles
+    const bool leader = (ct & 127) == 0;
+    const uint32_t stage = epi_base + (uint32_t)(wg * p.epi_nbuf) * (64u * 128u);
+    const uint32_t r0 = 16u * (uint32_t)q + ((uint32_t)lane >> 2);
+    uint32_t sbuf = 0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      int t = tile;
+      const int nt = t % p.tiles_n; t /= p.tiles_n;
+      const int ws = t % p.segs; t /= p.segs;
+      const int hp = t % p.hpairs; t /= p.hpairs;
+      const int b = t;
+      float acc[2][BN / 2];
+      rows_mma_tile<BN>(p, acc, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb, ita, itb, wg);
+      const int w0 = ws * 128 + wg * 64;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int h = hp * 2 + j;
+        long long pix[2], rpix[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int w = w0 + (int)r0 + 8 * hr;
+          pix[hr] = ((long long)b * p.H + h) * p.W + w;
+          rpix[hr] = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1)) : pix[hr];
+        }
+        epilogue_frag_tma<F, BN>(p.e, tmY, acc[j], nt * BN, w0, h, b, pix, rpix, alpha, stage, p.epi_nbuf, sbuf, 1u + wg, leader);
+      }
+    }
+    if (leader) bulk_wait_all();                 // staging tiles must outlive the last tensor store
+  }
 }
 
 template <int F>      // epilogue variant, see conv_epilogue.cuh
@@ -147,9 +183,8 @@ __global__ void __launch_bounds__(kRowsThreads, 1)
 conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmY, const RowsArgs p) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t epi_stage_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t acc_base = epi_stage_base + (p.use_tma ? (uint32_t)p.epi_bufs * kEpiStageBytes : 0u);
-  const uint32_t smem_base = acc_base + 128u * rows_acc_ld(p.BN);   // 1024-aligned: 128 rows x (16 mod 1024) B
+  const uint32_t epi_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // bf16 staging tiles, or fp32 accumulator rows (!use_tma)
+  const uint32_t smem_base = epi_base + rows_epi_bytes(p);              // 1024-aligned
   const uint32_t a_stage_bytes = 4 * kRowBufBytes;
   const uint32_t b_tile_bytes = (uint32_t)p.BN * 128u;
   const uint32_t a_base = smem_base;
@@ -182,6 +217,17 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     b = t;
   };
 
+  if (warp >= 4) {
+    reg_alloc<kConsumerRegs>();
+    switch (p.BN) {
+      case 16: rows_consumer<F, 16>(p, &tmY, epi_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
+      case 32: rows_consumer<F, 32>(p, &tmY, epi_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
+      case 64: rows_consumer<F, 64>(p, &tmY, epi_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
+      default: rows_consumer<F, 128>(p, &tmY, epi_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
+    }
+    return;
+  }
+  reg_dealloc<kProducerRegs>();     // the whole producer warpgroup, idle warps 1 and 3 included
   if (warp == 0) {
     if (lane == 0) {
       // ------------------------------------------------------------- A producer: four halo rows per K block
@@ -222,13 +268,6 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         }
       }
     }
-  } else if (warp >= 4) {
-    switch (p.BN) {
-      case 16: rows_consumer<F, 16>(p, &tmY, epi_stage_base, acc_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
-      case 32: rows_consumer<F, 32>(p, &tmY, epi_stage_base, acc_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
-      case 64: rows_consumer<F, 64>(p, &tmY, epi_stage_base, acc_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
-      default: rows_consumer<F, 128>(p, &tmY, epi_stage_base, acc_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
-    }
   }
 }
 
@@ -255,9 +294,12 @@ int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream) {
   const uint32_t resident_bytes = 9u * p.kblocks * b_tile;
   p.use_tma = (!d->y_fp32 && p.BN % 64 == 0 && d->y_cstride % 8 == 0 && (!d->residual || d->res_cstride % 8 == 0) &&
                (!d->mask || d->mask_cstride % 8 == 0)) ? 1 : 0;
-  p.epi_bufs = p.BN >= 128 ? 2 : 1;
-  const uint32_t fixed = 128u * rows_acc_ld(p.BN) + (p.use_tma ? p.epi_bufs * kEpiStageBytes : 0);
-  p.resident = (p.tiles_n == 1 && resident_bytes + a_stage + fixed <= budget) ? 1 : 0;
+  // two staging tiles per warpgroup (a chunk's store overlaps the next chunk's packing), one where that would cost the
+  // resident filter its second halo stage (C = 64: 72 KiB taps + 2 x 68 KiB halo + 16 KiB staging)
+  p.epi_nbuf = 2;
+  p.resident = (p.tiles_n == 1 && resident_bytes + a_stage + rows_epi_bytes(p) <= budget) ? 1 : 0;
+  if (p.resident && p.use_tma && resident_bytes + 2 * a_stage + rows_epi_bytes(p) > budget) p.epi_nbuf = 1;
+  const uint32_t fixed = rows_epi_bytes(p);
   if (p.resident) {
     p.a_stages = (int)((budget - resident_bytes - fixed) / a_stage);
     if (p.a_stages > 3) p.a_stages = 3;
@@ -283,12 +325,11 @@ int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream) {
   }
   CUtensorMap tmY = tmA;
   if (p.use_tma) {
-    rc = make_act_tmap(&tmY, d->y, d->B, d->H, d->W, d->Cout, d->y_cstride, 128, 1, 1);
+    rc = make_act_tmap(&tmY, d->y, d->B, d->H, d->W, d->Cout, d->y_cstride, 64, 1, 1);   // one warpgroup's 64 pixels
     if (rc) return rc;
   }
   const int nb = p.resident ? 1 : p.b_stages;
-  const size_t smem = (size_t)p.a_stages * a_stage + (p.resident ? resident_bytes : p.b_stages * b_tile) +
-                      (p.use_tma ? p.epi_bufs * kEpiStageBytes : 0) + 128u * rows_acc_ld(p.BN) + 1024 +
+  const size_t smem = (size_t)p.a_stages * a_stage + (p.resident ? resident_bytes : p.b_stages * b_tile) + fixed + 1024 +
                       8 * (2 * p.a_stages + 2 * nb);
   SGB_REQUIRE(smem <= 227u * 1024u);
   const int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
