@@ -176,6 +176,8 @@ __global__ void __launch_bounds__(256) sn_bwd_apply_kernel(const float* __restri
 // Batched variant: every spectrally-normalised layer of a network in three launches (blockIdx.y = layer).  The per-layer
 // launches above cost ~30 us each in dependent tiny kernels; a BigGAN-Deep generator has 150+ such layers per forward.
 // ---------------------------------------------------------------------------------------------------------------------
+// A block adds the (64-row x 256-column) tiles blockIdx.x, blockIdx.x + gridDim.x, ... of its layer: the grid is capped
+// (4096 blocks), and a layer may have more tiles than that (an SN linear 16384 -> 4160 has 4160).
 __global__ void __launch_bounds__(256) sn_wtu_batch_kernel(const sgb_sn_layer* __restrict__ table, float eps) {
   __shared__ float sh[32];
   __shared__ bool last;
@@ -185,23 +187,26 @@ __global__ void __launch_bounds__(256) sn_wtu_batch_kernel(const sgb_sn_layer* _
   const int col_blocks = (K + 255) / 256, rows_per_block = 64;
   const int row_blocks = (R + rows_per_block - 1) / rows_per_block;
   const unsigned total = (unsigned)col_blocks * row_blocks;
-  if (blockIdx.x >= total) return;
-  const int bx = blockIdx.x % col_blocks, by = blockIdx.x / col_blocks;
+  const unsigned nblk = min((unsigned)gridDim.x, total);    // blocks taking part in this layer (and in its ticket)
+  if (blockIdx.x >= nblk) return;
   const float* W = L.W;
   float* ws = L.ws;
-  const int c = bx * 256 + threadIdx.x;
-  const int r0 = by * rows_per_block, r1 = min(r0 + rows_per_block, R);
-  if (c < K) {
-    float acc = 0.f;
-    const float* wp = W + (size_t)r0 * K + c;
-    for (int r = r0; r < r1; ++r, wp += K) acc = fmaf(__ldg(wp), __ldg(L.u + r), acc);
-    atomicAdd(ws + c, acc);
+  for (unsigned tile = blockIdx.x; tile < total; tile += nblk) {
+    const int bx = (int)(tile % col_blocks), by = (int)(tile / col_blocks);
+    const int c = bx * 256 + threadIdx.x;
+    const int r0 = by * rows_per_block, r1 = min(r0 + rows_per_block, R);
+    if (c < K) {
+      float acc = 0.f;
+      const float* wp = W + (size_t)r0 * K + c;
+      for (int r = r0; r < r1; ++r, wp += K) acc = fmaf(__ldg(wp), __ldg(L.u + r), acc);
+      atomicAdd(ws + c, acc);
+    }
   }
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) {
     unsigned* ticket = reinterpret_cast<unsigned*>(ws + K + R);
-    last = (atomicAdd(ticket, 1u) == total - 1);
+    last = (atomicAdd(ticket, 1u) == nblk - 1);
     if (last) *ticket = 0u;
   }
   __syncthreads();
