@@ -466,16 +466,24 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
 // (8 KiB; a thread's pair of column block j goes to 16-byte unit j ^ (row & 7), conflict-free) and one thread issues the
 // TMA store of the box (64 ch, 64 px).  Per element the arithmetic is that of epilogue_tile_tma's piece(): acc * alpha,
 // + bias, fmaf(residual, rs, .), ReLU, mask, fmaf(post-mask residual, rs, .), bf16 pack -- the outputs are bit-identical.
-// ReLU bit planes are OR-reduced over the four lanes that share a row.  Residual and bf16 mask are read from global memory.
-//   pix / rpix : output / residual pixel of this thread's two rows.  stage: this warpgroup's first staging tile (1024-aligned),
-//   nbuf tiles used round-robin (sbuf = next one).  bar: named barrier of the warpgroup.
+// ReLU bit planes are OR-reduced over the four lanes that share a row.
+//   cc         : 64-channel chunk of the accumulator (compile-time after unrolling: the fragments stay in registers).
+//   pix / rpix : output / residual pixel of this thread's two rows; valid: the row lies inside the output (rows outside are
+//                clipped by the TMA store; their global loads read pixel 0 and their bit-plane words are not written).
+//   stage      : this warpgroup's first staging tile (1024-aligned), nbuf (1..4) tiles used round-robin (sbuf = next one).
+//   bar        : named barrier of the warpgroup.
+//   aux_tile   : F with kEpiAuxRes / kEpiAuxMask: the chunk's residual / mask box (SWIZZLE_128B, 128-byte rows) filled by the
+//                aux producer; arow = the box row of each of this thread's two rows.  Other variants read global memory.
+static constexpr uint32_t kFragStageBytes = 64 * 128;
+
 template <int F, int BN>
-__device__ __forceinline__ void epilogue_frag_tma(const EpiArgs& p, const CUtensorMap* tmY, const float (&acc)[BN / 2], int n0,
-                                                  int c1, int c2, int c3, const long long (&pix)[2], const long long (&rpix)[2],
-                                                  float alpha, uint32_t stage, int nbuf, uint32_t& sbuf, uint32_t bar, bool leader) {
-  static_assert(F < 0 || (F & (kEpiSmStats | kEpiSmApply | kEpiSmBwd | kEpiAuxRes | kEpiAuxMask)) == 0,
-                "softmax and aux-ring epilogues are served by epilogue_tile_tma");
-  constexpr uint32_t kFragStageBytes = 64 * 128;
+__device__ __forceinline__ void epilogue_frag_chunk(const EpiArgs& p, const CUtensorMap* tmY, const float (&acc)[BN / 2], int cc,
+                                                    int nbase, int c1, int c2, int c3, const long long (&pix)[2],
+                                                    const long long (&rpix)[2], const bool (&valid)[2], float alpha, uint32_t stage,
+                                                    int nbuf, uint32_t& sbuf, uint32_t bar, bool leader, uint32_t aux_tile = 0u,
+                                                    const uint32_t (&arow)[2] = {0u, 0u}) {
+  static_assert(F < 0 || (F & (kEpiSmStats | kEpiSmApply | kEpiSmBwd)) == 0, "softmax epilogues are served by epilogue_tile_tma");
+  constexpr int aux_kind = F < 0 ? 0 : ((F & kEpiAuxRes) ? 1 : ((F & kEpiAuxMask) ? 2 : 0));
   const bool has_bias = F < 0 ? p.bias != nullptr : (F & kEpiBias) != 0;
   const bool do_relu = F < 0 ? p.relu != 0 : (F & kEpiRelu) != 0;
   const bool res_pre = F < 0 ? (p.residual != nullptr && !p.res_after) : (F & kEpiResPre) != 0;
@@ -489,82 +497,102 @@ __device__ __forceinline__ void epilogue_frag_tma(const EpiArgs& p, const CUtens
   const long long nw = p.Cout >> 6;
   const uint32_t w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31, q = l & 3;
   const uint32_t r0 = 16u * w + (l >> 2);
+  const long long lpix[2] = {valid[0] ? pix[0] : 0ll, valid[1] ? pix[1] : 0ll};
+  const long long lrpix[2] = {valid[0] ? rpix[0] : 0ll, valid[1] ? rpix[1] : 0ll};
+  const uint32_t stage_cur = stage + sbuf * kFragStageBytes;
+  if (leader) {                                  // the store that last used this staging tile has finished reading it
+    if (nbuf == 1) bulk_wait_read0();
+    else if (nbuf == 2) bulk_wait_read1();
+    else if (nbuf == 3) bulk_wait_read2();
+    else bulk_wait_read3();
+  }
+  sbuf = (sbuf + 1u == (uint32_t)nbuf) ? 0u : sbuf + 1u;
+  named_bar_sync(bar, 128);
+  uint32_t mb[2][2] = {{0u, 0u}, {0u, 0u}}, ob[2][2] = {{0u, 0u}, {0u, 0u}};
+  if (use_mbits) {
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const uint2 m = __ldg(reinterpret_cast<const uint2*>(p.mask_bits) + lpix[hr] * nw + (nbase >> 6));
+      mb[hr][0] = m.x; mb[hr][1] = m.y;
+    }
+  }
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj) {
+    const int j = cc * 8 + jj;                   // 8-column block of the accumulator
+    const int n = nbase + 8 * jj + 2 * (int)q;
+    const bool in_c = full_c || nbase + 8 * jj < p.Cout;      // Cout % 8 == 0: a column block is all in or all out
+    const uint32_t bit = 8u * (jj & 3) + 2u * q;              // bit of column 0 of the pair in its 32-bit half of the word
+    float2 bb = make_float2(0.f, 0.f);
+    if (has_bias && in_c) bb = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      // this pair's 4 bytes in the aux box: 16-byte unit jj of row arow sits at jj ^ (arow & 7), conflict-free like the staging
+      const uint32_t aaddr = aux_tile + arow[hr] * 128u + ((((uint32_t)jj) ^ (arow[hr] & 7u)) << 4) + 4u * q;
+      float f0 = acc[4 * j + 2 * hr] * alpha, f1 = acc[4 * j + 2 * hr + 1] * alpha;
+      if (has_bias && in_c) { f0 += bb.x; f1 += bb.y; }
+      if (res_pre && in_c) {
+        const uint32_t r = aux_kind == 1 ? ld_shared_b32(aaddr)
+                                         : __ldg(reinterpret_cast<const unsigned int*>(p.residual + lrpix[hr] * p.res_cstride + n));
+        f0 = fmaf(bf16_bits_lo(r), rs, f0); f1 = fmaf(bf16_bits_hi(r), rs, f1);
+      }
+      if (do_relu) {
+        f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f);
+        if (emit_bits && !bits_from_packed) ob[hr][jj >> 2] |= ((f0 > 0.f) ? 1u : 0u) << bit | ((f1 > 0.f) ? 1u : 0u) << (bit + 1);
+      }
+      if (use_mbits) {
+        const uint32_t m = mb[hr][jj >> 2] >> bit;
+        f0 = (m & 1u) ? f0 : 0.f; f1 = (m & 2u) ? f1 : 0.f;
+      } else if (has_mask && in_c) {
+        const uint32_t m = aux_kind == 2 ? ld_shared_b32(aaddr)
+                                         : __ldg(reinterpret_cast<const unsigned int*>(p.mask + lpix[hr] * p.mask_cstride + n));
+        f0 = bf16_bits_lo(m) > 0.f ? f0 : 0.f; f1 = bf16_bits_hi(m) > 0.f ? f1 : 0.f;
+      }
+      if (res_post && in_c) {
+        const uint32_t r = aux_kind == 1 ? ld_shared_b32(aaddr)
+                                         : __ldg(reinterpret_cast<const unsigned int*>(p.residual + lrpix[hr] * p.res_cstride + n));
+        f0 = fmaf(bf16_bits_lo(r), rs, f0); f1 = fmaf(bf16_bits_hi(r), rs, f1);
+      }
+      const uint32_t pk = pack_bf16x2(f0, f1);
+      if (bits_from_packed) {                    // as positive_bits16_packed: a half is flagged iff it is not +0
+        const uint32_t t = pk + 0x7FFF7FFFu;
+        ob[hr][jj >> 2] |= ((t >> 15) & 1u) << bit | (t >> 31) << (bit + 1);
+      }
+      const uint32_t r = r0 + 8u * hr;
+      st_shared_b32(stage_cur + r * 128u + ((((uint32_t)jj) ^ (r & 7u)) << 4) + 4u * q, pk);
+    }
+  }
+  if (emit_bits) {
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        ob[hr][k] |= __shfl_xor_sync(0xffffffffu, ob[hr][k], 1);
+        ob[hr][k] |= __shfl_xor_sync(0xffffffffu, ob[hr][k], 2);
+      }
+      if (q == 0 && valid[hr]) reinterpret_cast<uint2*>(p.relu_bits)[pix[hr] * nw + (nbase >> 6)] = make_uint2(ob[hr][0], ob[hr][1]);
+    }
+  }
+  fence_proxy_async_smem();                      // generic-proxy smem writes -> visible to the TMA (async proxy)
+  named_bar_sync(bar, 128);
+  if (leader) {
+    tma_store_4d(tmY, stage_cur, nbase, c1, c2, c3);
+    bulk_commit();
+  }
+}
+
+// All 64-channel chunks of one 64-row accumulator block whose rows all lie inside the output (halo-row kernel).
+template <int F, int BN>
+__device__ __forceinline__ void epilogue_frag_tma(const EpiArgs& p, const CUtensorMap* tmY, const float (&acc)[BN / 2], int n0,
+                                                  int c1, int c2, int c3, const long long (&pix)[2], const long long (&rpix)[2],
+                                                  float alpha, uint32_t stage, int nbuf, uint32_t& sbuf, uint32_t bar, bool leader) {
+  static_assert(F < 0 || (F & (kEpiAuxRes | kEpiAuxMask)) == 0, "the aux ring is read by callers of epilogue_frag_chunk");
+  const bool full_c = F >= 0 && (F & kEpiFull) != 0;
+  const bool valid[2] = {true, true};
 #pragma unroll                                   // static accumulator indices: the fragments stay in registers
   for (int cc = 0; cc * 64 < BN; ++cc) {
     const int nbase = n0 + cc * 64;
     if (!full_c && nbase >= p.Cout) break;
-    const uint32_t stage_cur = stage + sbuf * kFragStageBytes;
-    if (leader) {                                // the store that last used this staging tile has finished reading it
-      if (nbuf == 1) bulk_wait_read0();
-      else bulk_wait_read1();
-    }
-    sbuf = (sbuf + 1u == (uint32_t)nbuf) ? 0u : sbuf + 1u;
-    named_bar_sync(bar, 128);
-    uint32_t mb[2][2] = {{0u, 0u}, {0u, 0u}}, ob[2][2] = {{0u, 0u}, {0u, 0u}};
-    if (use_mbits) {
-#pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-        const uint2 m = __ldg(reinterpret_cast<const uint2*>(p.mask_bits) + pix[hr] * nw + (nbase >> 6));
-        mb[hr][0] = m.x; mb[hr][1] = m.y;
-      }
-    }
-#pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-      const int j = cc * 8 + jj;                 // 8-column block of the accumulator
-      const int n = nbase + 8 * jj + 2 * (int)q;
-      const bool in_c = full_c || nbase + 8 * jj < p.Cout;      // Cout % 8 == 0: a column block is all in or all out
-      const uint32_t bit = 8u * (jj & 3) + 2u * q;              // bit of column 0 of the pair in its 32-bit half of the word
-      float2 bb = make_float2(0.f, 0.f);
-      if (has_bias && in_c) bb = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-#pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-        float f0 = acc[4 * j + 2 * hr] * alpha, f1 = acc[4 * j + 2 * hr + 1] * alpha;
-        if (has_bias && in_c) { f0 += bb.x; f1 += bb.y; }
-        if (res_pre && in_c) {
-          const uint32_t r = __ldg(reinterpret_cast<const unsigned int*>(p.residual + rpix[hr] * p.res_cstride + n));
-          f0 = fmaf(bf16_bits_lo(r), rs, f0); f1 = fmaf(bf16_bits_hi(r), rs, f1);
-        }
-        if (do_relu) {
-          f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f);
-          if (emit_bits && !bits_from_packed) ob[hr][jj >> 2] |= ((f0 > 0.f) ? 1u : 0u) << bit | ((f1 > 0.f) ? 1u : 0u) << (bit + 1);
-        }
-        if (use_mbits) {
-          const uint32_t m = mb[hr][jj >> 2] >> bit;
-          f0 = (m & 1u) ? f0 : 0.f; f1 = (m & 2u) ? f1 : 0.f;
-        } else if (has_mask && in_c) {
-          const uint32_t m = __ldg(reinterpret_cast<const unsigned int*>(p.mask + pix[hr] * p.mask_cstride + n));
-          f0 = bf16_bits_lo(m) > 0.f ? f0 : 0.f; f1 = bf16_bits_hi(m) > 0.f ? f1 : 0.f;
-        }
-        if (res_post && in_c) {
-          const uint32_t r = __ldg(reinterpret_cast<const unsigned int*>(p.residual + rpix[hr] * p.res_cstride + n));
-          f0 = fmaf(bf16_bits_lo(r), rs, f0); f1 = fmaf(bf16_bits_hi(r), rs, f1);
-        }
-        const uint32_t pk = pack_bf16x2(f0, f1);
-        if (bits_from_packed) {                  // as positive_bits16_packed: a half is flagged iff it is not +0
-          const uint32_t t = pk + 0x7FFF7FFFu;
-          ob[hr][jj >> 2] |= ((t >> 15) & 1u) << bit | (t >> 31) << (bit + 1);
-        }
-        const uint32_t r = r0 + 8u * hr;
-        st_shared_b32(stage_cur + r * 128u + ((((uint32_t)jj) ^ (r & 7u)) << 4) + 4u * q, pk);
-      }
-    }
-    if (emit_bits) {
-#pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-#pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          ob[hr][k] |= __shfl_xor_sync(0xffffffffu, ob[hr][k], 1);
-          ob[hr][k] |= __shfl_xor_sync(0xffffffffu, ob[hr][k], 2);
-        }
-        if (q == 0) reinterpret_cast<uint2*>(p.relu_bits)[pix[hr] * nw + (nbase >> 6)] = make_uint2(ob[hr][0], ob[hr][1]);
-      }
-    }
-    fence_proxy_async_smem();                    // generic-proxy smem writes -> visible to the TMA (async proxy)
-    named_bar_sync(bar, 128);
-    if (leader) {
-      tma_store_4d(tmY, stage_cur, nbase, c1, c2, c3);
-      bulk_commit();
-    }
+    epilogue_frag_chunk<F, BN>(p, tmY, acc, cc, nbase, c1, c2, c3, pix, rpix, valid, alpha, stage, nbuf, sbuf, bar, leader);
   }
 }
 

@@ -8,9 +8,15 @@
 //           A = dY tile(s), B = X tile(s): same boxes, consumed as MN-major operands (the pixel axis is K).
 //
 // One persistent CTA per SM, 3 warpgroups: warp 0 = TMA producer (one lane), warp 2 = auxiliary-operand producer (fprop),
-// warpgroups 1 and 2 = consumers.  Each consumer warpgroup owns 64 of the tile's 128 rows (wgmma M = 64) with its
-// accumulators in registers.  fprop: the consumers stage the finished accumulator tile in shared memory as fp32 rows and
-// then run the fused epilogue on it (one thread = one row); the producer meanwhile fills the operand ring for the next tile.
+// warpgroups 1 and 2 = consumers.  The producer warpgroup drops to 40 registers (setmaxnreg), the consumers rise to 232.
+// fprop, compile-time epilogue variants (all but the softmax ones): ping-pong.  Each consumer warpgroup owns whole tiles
+// (local tile i -> warpgroup i & 1), issues two m64 wgmmas per K step (rows 0..63 / 64..127, 128 accumulator registers at
+// BN = 128) and, once its main loop is done, hands the tensor cores to the other warpgroup (named barriers) and runs the fused
+// epilogue straight from its registers: per 64-channel chunk and 64-row half, bf16 pairs into its own staging tiles and one TMA
+// store; residual / mask boxes arrive through its own aux ring.  The operand ring stays one ring in tile order.
+// fprop, run-time flags and softmax variants: both warpgroups run every tile (64 rows each), stage the accumulator tile in
+// shared memory as fp32 rows and run the epilogue on it (one thread = one row).
+// wgrad: each consumer warpgroup owns 64 of the tile's 128 rows; fp32 red.adds straight from the accumulator registers.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "conv_epilogue.cuh"
@@ -90,17 +96,215 @@ __device__ __forceinline__ void fprop_mma_tile(const FpropArgs& p, uint32_t smem
   named_bar_sync(kAccBar, kConsumerThreads);
 }
 
+// ------------------------------------------------------------------------------------------------ fprop, ping-pong schedule
+// Compile-time epilogue variants other than the softmax ones: each consumer warpgroup owns whole 128-row tiles (local tile i
+// goes to warpgroup i & 1) and runs the epilogue straight from its registers while the other warpgroup issues its MMAs.
+__host__ __device__ constexpr bool fprop_is_pingpong(int f) { return f >= 0 && (f & (kEpiSmStats | kEpiSmApply | kEpiSmBwd)) == 0; }
+static constexpr uint32_t kTurnBar = 4;       // named barriers 4 / 5: warpgroup 0 / 1 may start its next mainloop
+
+// Main loop of one 128-row tile on one warpgroup: per 16-wide K step two m64 wgmmas (rows 0..63 -> acc[0], 64..127 -> acc[1])
+// against the same B tile.  it = the tile's first position in the operand ring.
+template <int BN>
+__device__ __forceinline__ void fprop_pp_mma(const FpropArgs& p, float (&acc)[2][BN / 2], uint32_t smem_base, uint32_t stage_bytes,
+                                             uint32_t bres_base, uint32_t b_bytes, uint32_t bar_base, uint32_t it) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
+  const bool b_mn = (p.w_mode == 2);
+  const int kiters = p.taps * p.kblocks;
+  const uint32_t lane = threadIdx.x & 31;
+  int prev = -1;
+  for (int k = 0; k < kiters; ++k, ++it) {
+    const int s = it % p.stages;
+    const uint32_t ph = (it / p.stages) & 1;
+    mbar_wait(bar_base + 8u * s, ph);
+    const uint32_t sa = smem_base + s * stage_bytes;
+    const uint64_t adesc = make_sdesc_sw128(sa, 16, 1024);                 // [128][64]; rows 64.. are 8 KiB further
+    const uint32_t sb = p.b_resident ? bres_base + (uint32_t)k * b_bytes : sa + kABytes;
+    wgmma_fence();
+    if (b_mn) {
+      const uint64_t bdesc = make_sdesc_sw128(sb, 8192, 1024);
+#pragma unroll
+      for (int kk = 0; kk < kBlockK / 16; ++kk)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          Wgmma<BN>::template mma<0, 1>(acc[h], adesc + 512 * h + 2 * kk, bdesc + 128 * kk, (k > 0 || kk > 0) ? 1u : 0u);
+    } else {
+      const uint64_t bdesc = make_sdesc_sw128(sb, 16, 1024);
+#pragma unroll
+      for (int kk = 0; kk < kBlockK / 16; ++kk)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          Wgmma<BN>::template mma<0, 0>(acc[h], adesc + 512 * h + 2 * kk, bdesc + 2 * kk, (k > 0 || kk > 0) ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();                          // the previous K block's MMAs have retired: its ring slot is free
+    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev)); }
+    prev = s;
+  }
+  wgmma_wait<0>();
+  acc_fence(acc[0]);
+  acc_fence(acc[1]);
+  __syncwarp();
+  if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev));
+}
+
+// One consumer warpgroup of the ping-pong schedule.  The two warpgroups' main loops take turns (named barriers kTurnBar + wg),
+// so warpgroup A's epilogue runs under warpgroup B's MMAs.  The epilogue stores the tile as two 64-row half boxes per
+// 64-channel chunk through this warpgroup's staging tiles; a residual / mask chunk arrives in this warpgroup's aux ring as one
+// box of the whole tile, read by both halves.
+template <int F, int BN>
+__device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUtensorMap* tmY, uint32_t smem_base, uint32_t stage_bytes,
+                                                  uint32_t bres_base, uint32_t b_bytes, uint32_t bar_base, uint32_t epi_stage_base,
+                                                  uint32_t aux_stage_base, int wg) {
+  constexpr int aux_kind = (F & kEpiAuxRes) ? 1 : ((F & kEpiAuxMask) ? 2 : 0);
+  const uint32_t w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const float alpha = p.e.alpha_ptr ? p.e.alpha * __ldg(p.e.alpha_ptr) : p.e.alpha;
+  // the half box splits the outermost non-unit dimension of (tw, th, nb): 0 = w, 1 = h, 2 = b
+  const int split = p.nb > 1 ? 2 : (p.th > 1 ? 1 : 0);
+  // tile coordinates and aux-box row of this thread's four rows: half h, fragment row hr -> tile row 64 h + 16 w + lane / 4 + 8 hr
+  int wi[2][2], hi[2][2], bi[2][2];
+  uint32_t arow[2][2];
+  const bool aux_half = aux_kind == 1 && p.e.res_up2;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int row = 64 * h + 16 * (int)w + (int)(lane >> 2) + 8 * hr;
+      wi[h][hr] = row % p.tw; hi[h][hr] = (row / p.tw) % p.th; bi[h][hr] = row / (p.tw * p.th);
+      arow[h][hr] = aux_half ? (uint32_t)((bi[h][hr] * p.aux_th + (p.aux_th == p.th ? hi[h][hr] : (hi[h][hr] >> 1))) * p.aux_tw + (wi[h][hr] >> 1))
+                             : (uint32_t)row;
+    }
+  const uint32_t stage = epi_stage_base + (uint32_t)(wg * p.epi_nbuf) * kFragStageBytes;
+  const uint32_t aux_ring = aux_stage_base + (uint32_t)(wg * p.aux_depth) * kEpiStageBytes;
+  const uint32_t aux_full0 = bar_base + 8u * (2 * p.stages + 1 + wg * p.aux_depth);
+  const uint32_t aux_empty0 = bar_base + 8u * (2 * p.stages + 1 + (2 + wg) * p.aux_depth);
+  const int kiters = p.taps * p.kblocks;
+  const int n_local = (p.num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // this CTA's tiles
+  uint32_t sbuf = 0, aux_cnt = 0;
+  if (p.b_resident) mbar_wait(bar_base + 8u * (2 * p.stages), 0);
+  for (int i = wg; i < n_local; i += 2) {
+    int t = (int)blockIdx.x + i * (int)gridDim.x;
+    const int nt = t % p.tiles_n; t /= p.tiles_n;
+    const int wt = t % p.tiles_w; t /= p.tiles_w;
+    const int ht = t % p.tiles_h; t /= p.tiles_h;
+    const int bt = t;
+    float acc[2][BN / 2];
+    if (i > 0) named_bar_sync(kTurnBar + wg, 256);          // the other warpgroup has issued tile i - 1
+    fprop_pp_mma<BN>(p, acc, smem_base, stage_bytes, bres_base, b_bytes, bar_base, (uint32_t)(i * kiters));
+    if (i + 1 < n_local) named_bar_arrive(kTurnBar + (wg ^ 1), 256);
+    long long pix[2][2], rpix[2][2];
+    bool valid[2][2];
+    int c1[2], c2[2], c3[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      c1[h] = wt * p.tw + (split == 0 ? h * (p.tw >> 1) : 0);
+      c2[h] = ht * p.th + (split == 1 ? h * (p.th >> 1) : 0);
+      c3[h] = bt * p.nb + (split == 2 ? h * (p.nb >> 1) : 0);
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int x = wt * p.tw + wi[h][hr], y = ht * p.th + hi[h][hr], b = bt * p.nb + bi[h][hr];
+        valid[h][hr] = x < p.W && y < p.H && b < p.B;
+        pix[h][hr] = ((long long)b * p.H + y) * p.W + x;
+        rpix[h][hr] = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (y >> 1)) * (p.W >> 1) + (x >> 1)) : pix[h][hr];
+      }
+    }
+#pragma unroll                                    // static accumulator indices: the fragments stay in registers
+    for (int cc = 0; cc * 64 < BN; ++cc) {
+      const int nbase = nt * BN + cc * 64;
+      if (nbase >= p.e.Cout) break;                 // (the aux producer skips the same chunks)
+      uint32_t aux_tile = 0u, aslot = 0u;
+      if constexpr (aux_kind != 0) {
+        aslot = aux_cnt % (uint32_t)p.aux_depth;
+        mbar_wait(aux_full0 + 8u * aslot, (aux_cnt / (uint32_t)p.aux_depth) & 1u);
+        aux_tile = aux_ring + aslot * kEpiStageBytes;
+        ++aux_cnt;
+      }
+      epilogue_frag_chunk<F, BN>(p.e, tmY, acc[0], cc, nbase, c1[0], c2[0], c3[0], pix[0], rpix[0], valid[0], alpha, stage,
+                                 p.epi_nbuf, sbuf, 1u + wg, leader, aux_tile, arow[0]);
+      epilogue_frag_chunk<F, BN>(p.e, tmY, acc[1], cc, nbase, c1[1], c2[1], c3[1], pix[1], rpix[1], valid[1], alpha, stage,
+                                 p.epi_nbuf, sbuf, 1u + wg, leader, aux_tile, arow[1]);
+      // every thread of the warpgroup is past its last read of the aux box (the barrier before the second half's store)
+      if (aux_kind != 0 && leader) mbar_arrive(aux_empty0 + 8u * aslot);
+    }
+  }
+  if (leader) bulk_wait_all();                    // staging tiles must outlive the last tensor store
+}
+
+// Staged-epilogue consumer (run-time flags and softmax variants): both warpgroups run the MMAs of every tile, stage the
+// accumulators in shared memory as fp32 rows, then run the epilogue on them.
+template <int F>
+__device__ __forceinline__ void fprop_staged_consumer(const FpropArgs& p, const CUtensorMap* tmY, uint32_t smem_base, uint32_t stage_bytes,
+                                                      uint32_t bres_base, uint32_t b_bytes, uint32_t bar_base, uint32_t epi_stage_base,
+                                                      uint32_t aux_stage_base, uint32_t acc_base, int wg) {
+  // Epilogue: team = which 64-channel chunks (even / odd) = consumer warpgroup, q = which 32 rows.
+  const int ct = threadIdx.x - 128;
+  const int lane = threadIdx.x & 31;
+  const int q = (ct >> 5) & 3;
+  const int team = wg;
+  const int row = q * 32 + lane;
+  const bool leader = (q == 0) && (lane == 0);
+  const int wi = row % p.tw, hi = (row / p.tw) % p.th, bi = row / (p.tw * p.th);
+  const bool vec_ok = epi_vec_ok(p.e);
+  const float alpha = p.e.alpha_ptr ? p.e.alpha * __ldg(p.e.alpha_ptr) : p.e.alpha;
+  const uint32_t stage = epi_stage_base + team * p.epi_nbuf * kEpiStageBytes;
+  const uint32_t t_row = acc_base + (uint32_t)row * acc_row_bytes(p.BN);
+  uint32_t aux_cnt = 0, sbuf = 0, it = 0;
+  EpiAux aux;
+  aux.kind = p.aux_kind; aux.ring = aux_stage_base + (uint32_t)(team * p.aux_depth) * kEpiStageBytes;
+  aux.full0 = bar_base + 8u * (2 * p.stages + 1 + team * p.aux_depth);
+  aux.empty0 = bar_base + 8u * (2 * p.stages + 1 + (2 + team) * p.aux_depth);
+  aux.depth = p.aux_depth; aux.cnt = &aux_cnt;
+  const bool aux_half = p.aux_kind == 1 && p.e.res_up2;
+  aux.arow = aux_half ? ((bi * p.aux_th + (p.aux_th == p.th ? hi : (hi >> 1))) * p.aux_tw + (wi >> 1)) : row;
+  if (p.b_resident) mbar_wait(bar_base + 8u * (2 * p.stages), 0);
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    int t = tile;
+    const int nt = t % p.tiles_n; t /= p.tiles_n;
+    const int wt = t % p.tiles_w; t /= p.tiles_w;
+    const int ht = t % p.tiles_h; t /= p.tiles_h;
+    const int bt = t;
+    const int n0 = nt * p.BN;
+    const int w = wt * p.tw + wi, h = ht * p.th + hi, b = bt * p.nb + bi;
+    const bool valid = (w < p.W) && (h < p.H) && (b < p.B) && (p.out_sub == 1 || (((w | h) & 1) == 0));
+    const long long pix = p.out_sub == 1 ? ((long long)b * p.H + h) * p.W + w
+                                         : ((long long)b * ((p.H + 1) >> 1) + (h >> 1)) * ((p.W + 1) >> 1) + (w >> 1);
+    const long long rpix = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1)) : pix;
+
+    switch (p.BN) {
+      case 16: fprop_mma_tile<16>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+      case 32: fprop_mma_tile<32>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+      case 64: fprop_mma_tile<64>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+      default: fprop_mma_tile<128>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+    }
+    if constexpr (F >= 0 && (F & kEpiSmStats) != 0) {
+      epilogue_tile_smstats(p.e, t_row, p.BN, n0, valid, pix, alpha, team, nt * 2 + team);
+    } else if (p.use_tma) {
+      epilogue_tile_tma<F>(p.e, tmY, t_row, p.BN, n0, wt * p.tw, ht * p.th, bt * p.nb, valid, pix, rpix, alpha, stage, team, row,
+                           leader, 2, p.aux_kind ? &aux : nullptr, p.epi_nbuf >= 2 ? &sbuf : nullptr, p.epi_nbuf);
+    } else if (team == 0) {
+      epilogue_row(p.e, t_row, p.BN, n0, valid, pix, rpix, alpha, vec_ok);
+    }
+  }
+  if (p.use_tma && leader) bulk_wait_all();   // staging tiles must outlive the last tensor store
+}
+
 template <int F>      // epilogue variant (conv_epilogue.cuh: kEpi* bits fixed at compile time; -1 = run-time flags)
 __global__ void __launch_bounds__(kThreads, 1)
 conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmAux, const FpropArgs p) {
+  constexpr bool pingpong = fprop_is_pingpong(F);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t epi_stage_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // staging tiles when use_tma
-  const uint32_t aux_stage_base = epi_stage_base + (p.use_tma ? 2u * p.epi_nbuf * kEpiStageBytes : 0u);   // + aux tiles when aux_kind
+  const uint32_t epi_bytes = p.use_tma ? 2u * p.epi_nbuf * (pingpong ? kFragStageBytes : kEpiStageBytes) : 0u;
+  const uint32_t aux_stage_base = epi_stage_base + epi_bytes;            // + aux tiles when aux_kind
   const uint32_t b_bytes = (uint32_t)p.BN * kBlockK * 2;  // same size for K-major [BN][64] and MN-major (BN/64) x [64][64]
   const uint32_t bres_base = aux_stage_base + (p.aux_kind ? 2u * p.aux_depth * kEpiStageBytes : 0u);     // resident weight tiles [tap][kb]
   const uint32_t acc_base = bres_base + (p.b_resident ? (uint32_t)(p.taps * p.kblocks) * b_bytes : 0u);  // fp32 accumulator rows
-  const uint32_t smem_base = acc_base + (uint32_t)kTileM * acc_row_bytes(p.BN);   // 1024-aligned: 128 rows x (16 mod 1024) B
+  // 1024-aligned: 128 rows x (16 mod 1024) B
+  const uint32_t smem_base = acc_base + (pingpong ? 0u : (uint32_t)kTileM * acc_row_bytes(p.BN));
   const uint32_t stage_bytes = kABytes + (p.b_resident ? 0u : b_bytes);  // multiple of 1024 because BN % 8 == 0 -> b_bytes % 1024 == 0
   const uint32_t bar_base = smem_base + (uint32_t)p.stages * stage_bytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
@@ -117,7 +321,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), kConsumerWarps);
+      mbar_init(empty_bar(s), pingpong ? kConsumerWarps / 2 : kConsumerWarps);   // ping-pong: one warpgroup per stage
     }
     for (int a = 0; a < 2; ++a)
       for (int sl = 0; sl < p.aux_depth; ++sl) { mbar_init(aux_full(a, sl), 1); mbar_init(aux_empty(a, sl), 1); }
@@ -127,9 +331,21 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   }
   __syncthreads();
 
+  if (warp >= 4) {
+    reg_alloc<kConsumerRegs>();
+    const int wg = (threadIdx.x - 128) >> 7;
+    if constexpr (pingpong) {
+      if (p.BN == 64) fprop_pp_consumer<F, 64>(p, &tmY, smem_base, stage_bytes, bres_base, b_bytes, bar_base, epi_stage_base, aux_stage_base, wg);
+      else fprop_pp_consumer<F, 128>(p, &tmY, smem_base, stage_bytes, bres_base, b_bytes, bar_base, epi_stage_base, aux_stage_base, wg);
+    } else {
+      fprop_staged_consumer<F>(p, &tmY, smem_base, stage_bytes, bres_base, b_bytes, bar_base, epi_stage_base, aux_stage_base, acc_base, wg);
+    }
+    return;
+  }
+  reg_dealloc<kProducerRegs>();     // the whole producer warpgroup, idle warps 1 and 3 included
   if (warp == 0) {
     if (lane == 0) {
-      // ------------------------------------------------------------- TMA producer
+      // ------------------------------------------------------------- TMA producer: one operand ring in tile order
       uint32_t it = 0;
       if (p.b_resident) {       // tiles_n == 1: the whole (small) filter is fetched once per CTA instead of once per tile
         mbar_arrive_expect_tx(bres_bar, (uint32_t)(p.taps * p.kblocks) * b_bytes);
@@ -169,11 +385,12 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   } else if (warp == 2) {
     if (lane == 0 && p.aux_kind) {
       // ------------------------------------------------------------- aux producer: residual / mask boxes, in the order the
-      // two epilogue teams consume their chunks (team = chunk & 1), up to aux_depth boxes ahead per team
+      // two rings are consumed (staged epilogue: team = chunk & 1; ping-pong: ring = local tile & 1), up to aux_depth boxes
+      // ahead per ring
       const bool half = p.aux_kind == 1 && p.e.res_up2;
       const uint32_t bytes = (uint32_t)(p.aux_tw * p.aux_th * p.nb) * 128u;
       uint32_t cnt[2] = {0u, 0u};
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      for (int tile = blockIdx.x, i = 0; tile < p.num_tiles; tile += gridDim.x, ++i) {
         int t = tile;
         const int nt = t % p.tiles_n; t /= p.tiles_n;
         const int wt = t % p.tiles_w; t /= p.tiles_w;
@@ -182,7 +399,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int cc = 0; cc * 64 < p.BN; ++cc) {
           const int nbase = nt * p.BN + cc * 64;
           if (nbase >= p.e.Cout) break;
-          const int team = cc & 1;
+          const int team = pingpong ? (i & 1) : (cc & 1);
           const uint32_t slot = cnt[team] % (uint32_t)p.aux_depth;
           mbar_wait(aux_empty(team, slot), ((cnt[team] / (uint32_t)p.aux_depth) & 1u) ^ 1u);
           mbar_arrive_expect_tx(aux_full(team, slot), bytes);
@@ -191,56 +408,6 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
-  } else if (warp >= 4) {
-    // --------------------------------------------------------------- consumers: MMA, then the epilogue on the staged tile.
-    // Epilogue: team = which 64-channel chunks (even / odd) = consumer warpgroup, q = which 32 rows.
-    const int ct = threadIdx.x - 128;
-    const int wg = ct >> 7;
-    const int q = (ct >> 5) & 3;
-    const int team = wg;
-    const int row = q * 32 + lane;
-    const bool leader = (q == 0) && (lane == 0);
-    const int wi = row % p.tw, hi = (row / p.tw) % p.th, bi = row / (p.tw * p.th);
-    const bool vec_ok = epi_vec_ok(p.e);
-    const float alpha = p.e.alpha_ptr ? p.e.alpha * __ldg(p.e.alpha_ptr) : p.e.alpha;
-    const uint32_t stage = epi_stage_base + team * p.epi_nbuf * kEpiStageBytes;
-    const uint32_t t_row = acc_base + (uint32_t)row * acc_row_bytes(p.BN);
-    uint32_t aux_cnt = 0, sbuf = 0, it = 0;
-    EpiAux aux;
-    aux.kind = p.aux_kind; aux.ring = aux_stage_base + (uint32_t)(team * p.aux_depth) * kEpiStageBytes;
-    aux.full0 = aux_full(team, 0); aux.empty0 = aux_empty(team, 0); aux.depth = p.aux_depth; aux.cnt = &aux_cnt;
-    const bool aux_half = p.aux_kind == 1 && p.e.res_up2;
-    aux.arow = aux_half ? ((bi * p.aux_th + (p.aux_th == p.th ? hi : (hi >> 1))) * p.aux_tw + (wi >> 1)) : row;
-    if (p.b_resident) mbar_wait(bres_bar, 0);
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      int t = tile;
-      const int nt = t % p.tiles_n; t /= p.tiles_n;
-      const int wt = t % p.tiles_w; t /= p.tiles_w;
-      const int ht = t % p.tiles_h; t /= p.tiles_h;
-      const int bt = t;
-      const int n0 = nt * p.BN;
-      const int w = wt * p.tw + wi, h = ht * p.th + hi, b = bt * p.nb + bi;
-      const bool valid = (w < p.W) && (h < p.H) && (b < p.B) && (p.out_sub == 1 || (((w | h) & 1) == 0));
-      const long long pix = p.out_sub == 1 ? ((long long)b * p.H + h) * p.W + w
-                                           : ((long long)b * ((p.H + 1) >> 1) + (h >> 1)) * ((p.W + 1) >> 1) + (w >> 1);
-      const long long rpix = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1)) : pix;
-
-      switch (p.BN) {
-        case 16: fprop_mma_tile<16>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
-        case 32: fprop_mma_tile<32>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
-        case 64: fprop_mma_tile<64>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
-        default: fprop_mma_tile<128>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
-      }
-      if constexpr (F >= 0 && (F & kEpiSmStats) != 0) {
-        epilogue_tile_smstats(p.e, t_row, p.BN, n0, valid, pix, alpha, team, nt * 2 + team);
-      } else if (p.use_tma) {
-        epilogue_tile_tma<F>(p.e, &tmY, t_row, p.BN, n0, wt * p.tw, ht * p.th, bt * p.nb, valid, pix, rpix, alpha, stage, team, row,
-                             leader, 2, p.aux_kind ? &aux : nullptr, p.epi_nbuf >= 2 ? &sbuf : nullptr, p.epi_nbuf);
-      } else if (team == 0) {
-        epilogue_row(p.e, t_row, p.BN, n0, valid, pix, rpix, alpha, vec_ok);
-      }
-    }
-    if (p.use_tma && leader) bulk_wait_all();   // staging tiles must outlive the last tensor store
   }
 }
 
@@ -439,8 +606,35 @@ int pick_bn(const sgb_conv_desc* d) {
   return BN;
 }
 
-// The staged TMA-store epilogue pays off on output-heavy layers only: K = taps * Cin up to this bound.
-static constexpr int kEpiTmaMaxK = 640;
+// The hot epilogue shapes of the training step get compile-time variants of the kernel; every other launch takes the
+// general kernel (F = -1, run-time flags).
+template <int... Fs>
+struct FpropVariants {
+  static constexpr bool has(int f) { return ((f == Fs) || ...); }
+  static int launch(int f, int grid, size_t smem, cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB,
+                    const CUtensorMap& tmY, const CUtensorMap& tmAux, const FpropArgs& p) {
+    int rc = 0;
+    const bool hit = ((f == Fs && ((rc = launch_kernel<conv_fprop_kernel<Fs>>(grid, kThreads, smem, stream, tmA, tmB, tmY, tmAux, p)),
+                                   true)) || ...);
+    return hit ? rc : launch_kernel<conv_fprop_kernel<-1>>(grid, kThreads, smem, stream, tmA, tmB, tmY, tmAux, p);
+  }
+};
+using FpropCompiled = FpropVariants<
+    kEpiFull,                                                          // dgrad / attention GEMMs
+    kEpiFull | kEpiBias,                                               // generator convs
+    kEpiFull | kEpiBias | kEpiRelu,                                    // discriminator convs (no backward expected)
+    kEpiFull | kEpiBias | kEpiRelu | kEpiBitsOut,                      // ... writing the ReLU bit plane
+    kEpiFull | kEpiResPre | kEpiAuxRes,                                // concat-skip dgrad
+    kEpiFull | kEpiBias | kEpiResPre | kEpiAuxRes,                     // block output + skip
+    kEpiFull | kEpiBias | kEpiRelu | kEpiResPre | kEpiAuxRes,          // ... with the next block's ReLU
+    kEpiFull | kEpiBias | kEpiRelu | kEpiResPre | kEpiAuxRes | kEpiBitsOut,
+    kEpiFull | kEpiMask | kEpiMaskBits,                                // dgrad through a ReLU (bit plane)
+    kEpiFull | kEpiMask | kEpiMaskBits | kEpiResPre | kEpiAuxRes,      // fused block entry (bit plane + pooled-skip gradient)
+    kEpiFull | kEpiMask | kEpiAuxMask,                                 // dgrad through a ReLU (bf16 mask tile)
+    kEpiFull | kEpiMask | kEpiResPre | kEpiAuxMask,                    // fused block entry (bf16 mask tile)
+    kEpiFull | kEpiSmStats,                                            // attention: row (max, sum exp) partials of theta . phi^T
+    kEpiFull | kEpiSmApply,                                            // attention: P = softmax(theta . phi^T) written directly
+    kEpiFull | kEpiSmBwd>;                                             // attention: dS = P * (do . g^T - delta)
 
 bool wgrad3x3_c64_eligible(const sgb_wgrad_desc* d);
 int launch_wgrad3x3_c64(const sgb_wgrad_desc* d, cudaStream_t stream);
@@ -500,8 +694,7 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   p.out_sub = d->out_sub == 2 ? 2 : 1;
   SGB_REQUIRE(p.out_sub == 1 || (!d->residual && !d->mask));
   p.use_tma = (p.out_sub == 1 && !d->y_fp32 && BN % 64 == 0 && d->Cout % 8 == 0 && d->y_cstride % 8 == 0 &&
-               (!d->residual || d->res_cstride % 8 == 0) && (!d->mask || d->mask_cstride % 8 == 0) &&
-               p.taps * d->Cin <= kEpiTmaMaxK) ? 1 : 0;
+               (!d->residual || d->res_cstride % 8 == 0) && (!d->mask || d->mask_cstride % 8 == 0)) ? 1 : 0;
   // auxiliary epilogue operand through TMA: exactly one of residual / mask, bf16 NHWC with 16-byte aligned channel stride
   p.aux_kind = 0; p.aux_tw = p.tw; p.aux_th = p.th;
   if (p.use_tma && (d->residual != nullptr || d->mask != nullptr)) {   // (mask_bits are 8-byte direct loads)
@@ -516,16 +709,30 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
     SGB_REQUIRE(p.use_tma);                                            // (the softmax variants exist only for the staged-store epilogue)
     if (d->sm_mode == 3) p.aux_kind = 3;                               // P tile of the softmax backward
   }
+  fill_epi(p.e, d);
+  p.e.sm_parts = 2 * p.tiles_n;
+  int f = p.use_tma ? epi_flags_of(p.e) : -1;
+  SGB_REQUIRE(!d->sm_mode || f == (kEpiFull | (d->sm_mode == 1 ? kEpiSmStats : d->sm_mode == 2 ? kEpiSmApply : kEpiSmBwd)));
+  if (f >= 0 && p.aux_kind == 1) f |= kEpiAuxRes;
+  if (f >= 0 && p.aux_kind == 2) f |= kEpiAuxMask;
+  if (!FpropCompiled::has(f)) f = -1;
+  // ping-pong variants: no fp32 accumulator staging; 8 KiB half-tile staging tiles per warpgroup.  Staged variants: fp32 rows
+  // of the whole tile plus 16 KiB staging tiles per epilogue team.
+  const bool pingpong = fprop_is_pingpong(f);
+  const int epi_tile_kb = pingpong ? (int)(kFragStageBytes / 1024) : (int)(kEpiStageBytes / 1024);
+  const int acc_kb = pingpong ? 0 : (int)(kTileM * acc_row_bytes(BN) / 1024);
   // short-K layers (one or two K blocks per tile) are store bound: their (small) filter stays resident in shared memory and the
   // space of the B halves of the ring buys more staging tiles per epilogue team = more store bytes in flight
   const uint32_t b_tile = (uint32_t)BN * kBlockK * 2;
   const int kt = p.taps * p.kblocks;
   p.b_resident = (d->w_mode == 0 && p.tiles_n == 1 && kt <= 2 && kt * b_tile <= 64u * 1024u) ? 1 : 0;
   const uint32_t stage_bytes = kABytes + (p.b_resident ? 0u : b_tile);
-  p.epi_nbuf = (p.use_tma && kt <= 2) ? 2 : 1;
+  p.epi_nbuf = !p.use_tma ? 1 : pingpong ? (kt <= 2 ? 4 : 2) : (kt <= 2 ? 2 : 1);
   p.aux_depth = p.aux_kind ? 2 : 1;
-  const int acc_kb = (int)(kTileM * acc_row_bytes(BN) / 1024);
-  auto ring_kb = [&](int nbuf) { return 216 - acc_kb - (p.use_tma ? 32 * nbuf : 0) - (p.aux_kind ? 32 * p.aux_depth : 0) - (p.b_resident ? (int)(kt * b_tile / 1024) : 0); };
+  auto ring_kb = [&](int nbuf) {
+    return 216 - acc_kb - (p.use_tma ? 2 * epi_tile_kb * nbuf : 0) - (p.aux_kind ? 32 * p.aux_depth : 0) -
+           (p.b_resident ? (int)(kt * b_tile / 1024) : 0);
+  };
   // keep >= 3 operand ring stages: give back aux depth first, then staging tiles
   while (p.aux_kind && p.aux_depth > 1 && ring_kb(p.epi_nbuf) * 1024 < (int)(3 * stage_bytes)) --p.aux_depth;
   while (p.epi_nbuf > 1 && ring_kb(p.epi_nbuf) * 1024 < (int)(3 * stage_bytes)) --p.epi_nbuf;
@@ -533,8 +740,6 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   if (stages > 8) stages = 8;
   if (stages < 2) stages = 2;
   p.stages = stages;
-  fill_epi(p.e, d);
-  p.e.sm_parts = 2 * p.tiles_n;
 
   CUtensorMap tmA, tmB;
   int rc = make_act_tmap(&tmA, d->x, d->B, Hin, Win, d->Cin, d->x_cstride, p.tw, p.th, p.nb);
@@ -558,7 +763,10 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   if (rc) return rc;
   CUtensorMap tmY = tmA;
   if (p.use_tma) {
-    rc = make_act_tmap(&tmY, d->y, d->B, d->H, d->W, d->Cout, d->y_cstride, p.tw, p.th, p.nb);
+    // ping-pong: one store per 64-row half of the tile, whose box halves the outermost non-unit dimension of (tw, th, nb)
+    const int split = p.nb > 1 ? 2 : (p.th > 1 ? 1 : 0);
+    rc = make_act_tmap(&tmY, d->y, d->B, d->H, d->W, d->Cout, d->y_cstride, pingpong && split == 0 ? p.tw / 2 : p.tw,
+                       pingpong && split == 1 ? p.th / 2 : p.th, pingpong && split == 2 ? p.nb / 2 : p.nb);
     if (rc) return rc;
   }
   CUtensorMap tmAux = tmA;
@@ -569,36 +777,12 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
     rc = make_act_tmap(&tmAux, ap, d->B, half ? d->H / 2 : d->H, half ? d->W / 2 : d->W, d->Cout, acs, p.aux_tw, p.aux_th, p.nb);
     if (rc) return rc;
   }
-  const size_t smem = (size_t)stages * stage_bytes + (p.use_tma ? 2 * p.epi_nbuf * kEpiStageBytes : 0) + (p.aux_kind ? 2 * p.aux_depth * kEpiStageBytes : 0) +
-                      (p.b_resident ? (size_t)kt * b_tile : 0) + (size_t)kTileM * acc_row_bytes(BN) + 1024 + 8 * (2 * stages + 1 + 4 * 3);
+  const size_t smem = (size_t)stages * stage_bytes + (p.use_tma ? 2 * p.epi_nbuf * epi_tile_kb * 1024 : 0) +
+                      (p.aux_kind ? 2 * p.aux_depth * kEpiStageBytes : 0) + (p.b_resident ? (size_t)kt * b_tile : 0) +
+                      (pingpong ? 0 : (size_t)kTileM * acc_row_bytes(BN)) + 1024 + 8 * (2 * stages + 1 + 4 * 3);
   SGB_REQUIRE(smem <= 227u * 1024u);
   int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
-  // the hot epilogue shapes of the training step get compile-time variants; everything else takes the general kernel
-  int f = p.use_tma ? epi_flags_of(p.e) : -1;
-  SGB_REQUIRE(!d->sm_mode || f == (kEpiFull | (d->sm_mode == 1 ? kEpiSmStats : d->sm_mode == 2 ? kEpiSmApply : kEpiSmBwd)));
-  if (f >= 0 && p.aux_kind == 1) f |= kEpiAuxRes;
-  if (f >= 0 && p.aux_kind == 2) f |= kEpiAuxMask;
-#define SGB_FPROP_CASE(FLAGS) \
-  case (FLAGS): return launch_kernel<conv_fprop_kernel<(FLAGS)>>(grid, kThreads, smem, stream, tmA, tmB, tmY, tmAux, p);
-  switch (f) {
-    SGB_FPROP_CASE(kEpiFull)                                                          // dgrad / attention GEMMs
-    SGB_FPROP_CASE(kEpiFull | kEpiBias)                                               // generator convs
-    SGB_FPROP_CASE(kEpiFull | kEpiBias | kEpiRelu)                                    // discriminator convs (no backward expected)
-    SGB_FPROP_CASE(kEpiFull | kEpiBias | kEpiRelu | kEpiBitsOut)                      // ... writing the ReLU bit plane
-    SGB_FPROP_CASE(kEpiFull | kEpiResPre | kEpiAuxRes)                                // concat-skip dgrad
-    SGB_FPROP_CASE(kEpiFull | kEpiBias | kEpiResPre | kEpiAuxRes)                     // block output + skip
-    SGB_FPROP_CASE(kEpiFull | kEpiBias | kEpiRelu | kEpiResPre | kEpiAuxRes)          // ... with the next block's ReLU
-    SGB_FPROP_CASE(kEpiFull | kEpiBias | kEpiRelu | kEpiResPre | kEpiAuxRes | kEpiBitsOut)
-    SGB_FPROP_CASE(kEpiFull | kEpiMask | kEpiMaskBits)                                // dgrad through a ReLU (bit plane)
-    SGB_FPROP_CASE(kEpiFull | kEpiMask | kEpiMaskBits | kEpiResPre | kEpiAuxRes)      // fused block entry (bit plane + pooled-skip gradient)
-    SGB_FPROP_CASE(kEpiFull | kEpiMask | kEpiAuxMask)                                 // dgrad through a ReLU (bf16 mask tile)
-    SGB_FPROP_CASE(kEpiFull | kEpiMask | kEpiResPre | kEpiAuxMask)                    // fused block entry (bf16 mask tile)
-    SGB_FPROP_CASE(kEpiFull | kEpiSmStats)                                            // attention: row (max, sum exp) partials of theta . phi^T
-    SGB_FPROP_CASE(kEpiFull | kEpiSmApply)                                            // attention: P = softmax(theta . phi^T) written directly
-    SGB_FPROP_CASE(kEpiFull | kEpiSmBwd)                                              // attention: dS = P * (do . g^T - delta)
-    default: return launch_kernel<conv_fprop_kernel<-1>>(grid, kThreads, smem, stream, tmA, tmB, tmY, tmAux, p);
-  }
-#undef SGB_FPROP_CASE
+  return FpropCompiled::launch(f, grid, smem, stream, tmA, tmB, tmY, tmAux, p);
 }
 
 extern "C" int sgb_conv_wgrad_fuses_dbias(const sgb_wgrad_desc* d) {
