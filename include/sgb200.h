@@ -224,7 +224,7 @@ int sgb_bn_bwd_apply(const void* dy, int64_t dy_cstride, const void* x, int64_t 
 /* out = act(a*[*a_dev]*x + b*y), then masked by (mask > 0) if mask; act 0 none / 1 relu. */
 int sgb_axpby(const void* x, int64_t xs, const void* y, int64_t ys, const void* mask, int64_t ms, void* out, int64_t os,
               int64_t npix, int32_t C, float a, const float* a_dev, float b, int32_t act, sgb_stream_t stream);
-/* 2x2 pooling to [B,Ho,Wo,C]; mode 0 average, 1 max. */
+/* 2x2 pooling to [B,Ho,Wo,C]; mode 0 average, 1 max, 2 sum (the gradient of a nearest x2 up-sampled residual). */
 int sgb_pool2_fwd(const void* x, int64_t xs, void* y, int64_t ys, int32_t B, int32_t Ho, int32_t Wo, int32_t C, int32_t mode,
                   sgb_stream_t stream);
 /* dx = pool2 backward of dy (+ add) (masked by relu_src > 0); x needed for max (first max in scan order wins).

@@ -68,7 +68,7 @@ __global__ void __launch_bounds__(256) axpby_kernel(const bf16* __restrict__ x, 
   }
 }
 
-// 2x2 pooling.  mode 0: average, 1: max.  One thread = 8 channels of one OUTPUT pixel.
+// 2x2 pooling.  mode 0: average, 1: max, 2: sum.  One thread = 8 channels of one OUTPUT pixel.
 __global__ void __launch_bounds__(256) pool2_fwd_kernel(const bf16* __restrict__ x, long long xs, bf16* __restrict__ y,
                                                          long long ys, int B, int Ho, int Wo, int C, int mode) {
   const int VG = C >> 3;

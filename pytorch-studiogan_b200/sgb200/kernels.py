@@ -309,7 +309,7 @@ def axpby(x, y=None, a=1.0, b=1.0, a_dev=None, mask=None, relu=False, out=None):
 
 
 def pool2_fwd(x, mode, out=None):
-    """mode 0 average, 1 max (2x2, stride 2)."""
+    """mode 0 average, 1 max, 2 sum (2x2, stride 2).  Sum is the gradient of a nearest x2 up-sampled residual."""
     B, C, H, W, xs = geom(x)
     if out is None:
         out = empty_nhwc(B, C, H // 2, W // 2, x.device)
