@@ -1,13 +1,20 @@
-// Fused conv epilogue shared by the wgmma conv kernels: accumulator row (staged in shared memory) -> alpha, bias, residual (optionally read
-// from a half-resolution tensor = nearest x2 upsample), ReLU, ReLU-mask, post-mask residual -> bf16 / fp32 NHWC store.
+// Fused conv epilogue shared by the wgmma conv kernels: accumulator -> alpha, bias, residual (optionally read from a
+// half-resolution tensor = nearest x2 upsample), ReLU, ReLU-mask, post-mask residual -> bf16 / fp32 NHWC store.
+// The questions of a variant are EpiOps<F>; the TMA-store epilogues share the arithmetic epi_pair (one bf16 pair of channels)
+// and only differ in where they load its operands from:
+//   epilogue_tile_tma  : fp32 accumulator rows staged in shared memory, aux tile in shared memory (run-time flags, softmax)
+//   epilogue_frag_chunk: straight from the wgmma accumulator registers
+// epilogue_row (direct stores, fp32 outputs, ragged channel tails) keeps 16-wide blocks per question: with run-time flags,
+// per-pair tests of each question are if-converted into selects on every element.
 #pragma once
 #include "common.cuh"
 #include "ptx.cuh"
+#include <type_traits>
 
 namespace sgb {
 
 struct EpiArgs {
-  int H, W, Cout;
+  int Cout;
   float alpha;
   const float* alpha_ptr;
   const float* bias;
@@ -28,31 +35,63 @@ struct EpiArgs {
   const float* sm_delta;      // [rows]
 };
 
-// 16 accumulator values -> 16 mask bits (value > 0)
-__device__ __forceinline__ uint32_t positive_bits16(const float (&f)[16]) {
-  uint32_t b = 0u;
-#pragma unroll
-  for (int j = 0; j < 16; ++j) b |= (f[j] > 0.f) ? (1u << j) : 0u;
-  return b;
+// Compile-time epilogue variants.  The per-piece loops run on 2 warps per scheduler with little latency hiding, so every
+// run-time test of "is there a bias / residual / mask / ragged channel tail" costs issue slots on the critical path of the
+// memory-bound layers (~150 SASS instructions per 16-column piece).  F >= 0 fixes those questions at compile time (bit 0
+// bias, 1 ReLU, 2 residual before the activation, 3 residual after the mask, 4 mask, 5 Cout % 64 == 0 and every 16-byte
+// alignment holds); F < 0 is the fully general run-time version.
+static constexpr int kEpiBias = 1, kEpiRelu = 2, kEpiResPre = 4, kEpiResPost = 8, kEpiMask = 16, kEpiFull = 32;
+// ... bit 6: the mask is a bit plane (mask_bits), 7 / 8: the residual / the bf16 mask tile arrives through the aux TMA ring,
+// 9: the ReLU epilogue also writes its bit plane (relu_bits).  In the fused block-entry dgrad (mask + residual), with these
+// three questions left to run time the compiler if-converts both sides of each and the piece loop issues 12 instructions per
+// output element (the bias-only variant: 2).
+static constexpr int kEpiMaskBits = 64, kEpiAuxRes = 128, kEpiAuxMask = 256, kEpiBitsOut = 512;
+// attention: bit 10 softmax statistics (no store), 11 softmax apply, 12 softmax backward (P tile through the aux ring)
+static constexpr int kEpiSmStats = 1024, kEpiSmApply = 2048, kEpiSmBwd = 4096;
+
+__host__ __device__ inline int epi_flags_of(const EpiArgs& p) {
+  int f = 0;
+  if (p.bias) f |= kEpiBias;
+  if (p.relu) f |= kEpiRelu;
+  if (p.residual) f |= p.res_after ? kEpiResPost : kEpiResPre;
+  if (p.mask || p.mask_bits) f |= kEpiMask;
+  if (p.mask_bits) f |= kEpiMaskBits;
+  if (p.relu && p.relu_bits) f |= kEpiBitsOut;
+  if (p.Cout % 64 == 0) f |= kEpiFull;
+  if (p.sm_mode == 1) f |= kEpiSmStats;
+  if (p.sm_mode == 2) f |= kEpiSmApply;
+  if (p.sm_mode == 3) f |= kEpiSmBwd;
+  return f;
 }
-// The same 16 bits from the PACKED bf16 pairs of a post-ReLU piece (every half is +0 or a positive value <= 0x7F80): adding
-// 0x7FFF to a half sets its bit 15 iff it is non-zero without carrying into its neighbour; PRMT gathers the four flag bytes of
-// two words, one multiply moves the four flags into a nibble.  27 integer instructions per piece instead of 40
-// (FSETP + SEL per element + adds) -- the bit plane is paid for by write-bound layers.
-__device__ __forceinline__ uint32_t positive_bits16_packed(const uint32_t (&w)[8]) {
-  uint32_t bits = 0u;
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const uint32_t ta = w[2 * k] + 0x7FFF7FFFu, tb = w[2 * k + 1] + 0x7FFF7FFFu;
-    const uint32_t flags = __byte_perm(ta, tb, 0x7531) & 0x80808080u;      // bits 7 / 15 / 23 / 31 = elements 4k .. 4k+3
-    bits |= ((flags * 0x00204081u) >> 28) << (4 * k);
+
+// The compiled variants of a kernel: launch(std::integral_constant<int, F>) runs variant F, or F = -1 (run-time flags) when f
+// is not one of them.
+template <int... Fs>
+struct EpiVariants {
+  static constexpr bool has(int f) { return ((f == Fs) || ...); }
+  template <class Launch>
+  static int launch(int f, Launch&& run) {
+    int rc = 0;
+    const bool hit = ((f == Fs && ((rc = run(std::integral_constant<int, Fs>{})), true)) || ...);
+    return hit ? rc : run(std::integral_constant<int, -1>{});
   }
-  return bits;
-}
-__device__ __forceinline__ void apply_bits16(float (&f)[16], uint32_t mb) {
-#pragma unroll
-  for (int j = 0; j < 16; ++j) f[j] = ((mb >> j) & 1u) ? f[j] : 0.f;
-}
+};
+
+// The questions of epilogue variant F: fixed at compile time for F >= 0, read from the arguments for F < 0.
+template <int F>
+struct EpiOps {
+  bool bias, relu, res_pre, res_post, mask, mask_bits, bits_out;
+  bool full_c;                                   // no channel-tail tests (F >= 0 only)
+  __device__ __forceinline__ explicit EpiOps(const EpiArgs& p)
+      : bias(F < 0 ? p.bias != nullptr : (F & kEpiBias) != 0),
+        relu(F < 0 ? p.relu != 0 : (F & kEpiRelu) != 0),
+        res_pre(F < 0 ? (p.residual != nullptr && !p.res_after) : (F & kEpiResPre) != 0),
+        res_post(F < 0 ? (p.residual != nullptr && p.res_after) : (F & kEpiResPost) != 0),
+        mask(F < 0 ? (p.mask != nullptr || p.mask_bits != nullptr) : (F & kEpiMask) != 0),
+        mask_bits(F < 0 ? p.mask_bits != nullptr : (F & kEpiMaskBits) != 0),
+        bits_out(F < 0 ? (p.relu != 0 && p.relu_bits != nullptr) : (F & kEpiBitsOut) != 0),
+        full_c(F >= 0 && (F & kEpiFull) != 0) {}
+};
 
 __device__ __forceinline__ float bf16_bits_lo(uint32_t u) { return __uint_as_float(u << 16); }
 __device__ __forceinline__ float bf16_bits_hi(uint32_t u) { return __uint_as_float(u & 0xFFFF0000u); }
@@ -61,9 +100,52 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&t);
 }
 
+// The arithmetic that follows acc * alpha, for two adjacent channels (c, c + 1): + bias, fmaf(residual, rs, .), ReLU, mask,
+// fmaf(post-mask residual, rs, .).  res / msk: the packed bf16 residual / mask pair (low half = channel c); mbits: the pair's
+// two mask bits (bit plane).  pos: bit 0 / 1 set iff the ReLU output of channel c / c + 1 is positive.
+template <int F>
+__device__ __forceinline__ float2 epi_pair(const EpiOps<F>& op, float f0, float f1, float2 b, uint32_t res, uint32_t msk,
+                                           uint32_t mbits, float rs, uint32_t& pos) {
+  pos = 0u;
+  if (op.bias) { f0 += b.x; f1 += b.y; }
+  if (op.res_pre) { f0 = fmaf(bf16_bits_lo(res), rs, f0); f1 = fmaf(bf16_bits_hi(res), rs, f1); }
+  if (op.relu) {
+    f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f);
+    pos = ((f0 > 0.f) ? 1u : 0u) | ((f1 > 0.f) ? 2u : 0u);
+  }
+  if (op.mask_bits) {
+    f0 = (mbits & 1u) ? f0 : 0.f; f1 = (mbits & 2u) ? f1 : 0.f;
+  } else if (op.mask) {
+    f0 = bf16_bits_lo(msk) > 0.f ? f0 : 0.f; f1 = bf16_bits_hi(msk) > 0.f ? f1 : 0.f;
+  }
+  if (op.res_post) { f0 = fmaf(bf16_bits_lo(res), rs, f0); f1 = fmaf(bf16_bits_hi(res), rs, f1); }
+  return make_float2(f0, f1);
+}
+
+// alpha, scaled by *alpha_ptr when it is given
+__device__ __forceinline__ float epi_alpha(const EpiArgs& p) { return p.alpha_ptr ? p.alpha * __ldg(p.alpha_ptr) : p.alpha; }
+
+// Residual pixel of output pixel pix = (b, h, w) of an H x W map: pix itself, or (res_up2) its nearest-x2 source pixel in the
+// H/2 x W/2 residual.
+__device__ __forceinline__ long long epi_rpix(const EpiArgs& p, int b, int h, int w, int H, int W, long long pix) {
+  return p.res_up2 ? (((long long)b * (H >> 1) + (h >> 1)) * (W >> 1) + (w >> 1)) : pix;
+}
+
 __device__ __forceinline__ bool epi_vec_ok(const EpiArgs& p) {
   return (p.Cout % 8 == 0) && (p.y_cstride % 8 == 0) && (p.residual == nullptr || p.res_cstride % 8 == 0) &&
          (p.mask == nullptr || p.mask_cstride % 8 == 0);
+}
+
+// 16 accumulator values -> 16 mask bits (value > 0)
+__device__ __forceinline__ uint32_t positive_bits16(const float (&f)[16]) {
+  uint32_t b = 0u;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) b |= (f[j] > 0.f) ? (1u << j) : 0u;
+  return b;
+}
+__device__ __forceinline__ void apply_bits16(float (&f)[16], uint32_t mb) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j) f[j] = ((mb >> j) & 1u) ? f[j] : 0.f;
 }
 
 // One thread = one accumulator row.  t_row: shared-memory address of this thread's accumulator row (acc_store layout);
@@ -201,37 +283,13 @@ __device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
 }
 static constexpr int kEpiStageBytes = 128 * 128;  // one 128-row x 64-channel bf16 chunk
 
-__device__ __forceinline__ bool epi_use_tma(const EpiArgs& p, int BN) {
-  return !p.y_fp32 && (BN % 64 == 0) && epi_vec_ok(p);
-}
-
-// Compile-time epilogue variants.  The per-piece loop below runs on 2 warps per scheduler with little latency hiding, so
-// every run-time test of "is there a bias / residual / mask / ragged channel tail" costs issue slots on the critical path of
-// the memory-bound layers (~150 SASS instructions per 16-column piece).  F >= 0 fixes those questions at compile
-// time (bit 0 bias, 1 ReLU, 2 residual before the activation, 3 residual after the mask, 4 mask, 5 Cout % 64 == 0 and every
-// 16-byte alignment holds); F < 0 is the fully general run-time version.
-static constexpr int kEpiBias = 1, kEpiRelu = 2, kEpiResPre = 4, kEpiResPost = 8, kEpiMask = 16, kEpiFull = 32;
-// ... bit 6: the mask is a bit plane (mask_bits), 7 / 8: the residual / the bf16 mask tile arrives through the aux TMA ring,
-// 9: the ReLU epilogue also writes its bit plane (relu_bits).  In the fused block-entry dgrad (mask + residual), with these
-// three questions left to run time the compiler if-converts both sides of each and the piece loop issues 12 instructions per
-// output element (the bias-only variant: 2).
-static constexpr int kEpiMaskBits = 64, kEpiAuxRes = 128, kEpiAuxMask = 256, kEpiBitsOut = 512;
-// attention: bit 10 softmax statistics (no store), 11 softmax apply, 12 softmax backward (P tile through the aux ring)
-static constexpr int kEpiSmStats = 1024, kEpiSmApply = 2048, kEpiSmBwd = 4096;
-
-__host__ __device__ inline int epi_flags_of(const EpiArgs& p) {
-  int f = 0;
-  if (p.bias) f |= kEpiBias;
-  if (p.relu) f |= kEpiRelu;
-  if (p.residual) f |= p.res_after ? kEpiResPost : kEpiResPre;
-  if (p.mask || p.mask_bits) f |= kEpiMask;
-  if (p.mask_bits) f |= kEpiMaskBits;
-  if (p.relu && p.relu_bits) f |= kEpiBitsOut;
-  if (p.Cout % 64 == 0) f |= kEpiFull;
-  if (p.sm_mode == 1) f |= kEpiSmStats;
-  if (p.sm_mode == 2) f |= kEpiSmApply;
-  if (p.sm_mode == 3) f |= kEpiSmBwd;
-  return f;
+// The next of a team's nbuf (1..4) staging tiles, used round-robin (sbuf = its index), so a chunk only waits for the store
+// issued nbuf chunks ago: the latency of the previous tensor stores is off the critical path and more bytes are in flight.
+__device__ __forceinline__ uint32_t epi_stage_next(uint32_t stage, uint32_t tile_bytes, int nbuf, uint32_t& sbuf, bool leader) {
+  const uint32_t cur = stage + sbuf * tile_bytes;
+  if (leader) bulk_wait_read(nbuf);              // the store that last used this staging tile has finished reading it
+  sbuf = (sbuf + 1u == (uint32_t)nbuf) ? 0u : sbuf + 1u;
+  return cur;
 }
 
 // 2^x on the SFU (ex2.approx: 2^-22 relative error, far below the bf16 rounding of the softmax output); the accurate exp2f
@@ -262,8 +320,8 @@ __device__ __forceinline__ void epilogue_tile_smstats(const EpiArgs& p, uint32_t
         for (int j = 0; j < 16; ++j) pm = fmaxf(pm, __uint_as_float(v[q][j]) * alpha);
       const float mn = fmaxf(m, pm);
       float acc = 0.f;
-#pragma unroll
       const float a2 = alpha * kLog2e, mn2 = -mn * kLog2e;
+#pragma unroll
       for (int q = 0; q < 2; ++q)
 #pragma unroll
         for (int j = 0; j < 16; ++j) acc += fast_ex2(fmaf(__uint_as_float(v[q][j]), a2, mn2));
@@ -277,15 +335,18 @@ __device__ __forceinline__ void epilogue_tile_smstats(const EpiArgs& p, uint32_t
   }
 }
 
+// Staged epilogue of the run-time general kernel (F = -1) and of the softmax apply / backward variants.
 // t_row : shared-memory address of this thread's accumulator row (first column of the accumulator).
 // c1..c3: box coordinates (w0, h0, b0) of the tile in the output tensor map; channel coordinate = n0 + chunk * 64.
-// stage : this team's staging buffer (1024-byte aligned).  team in {0,1}; row = accumulator row of this thread.
+// stage : this team's first staging tile (1024-byte aligned), nbuf tiles used round-robin (sbuf = next one).
+// team in {0,1}; row = accumulator row of this thread.  aux: the team's aux ring, or nullptr.
 // A thread converts all four 16-column pieces of its row of the chunk; a team is 4 warps.
 template <int F>
 __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtensorMap* tmY, uint32_t t_row, int BN, int n0,
                                                   int c1, int c2, int c3, bool valid, long long pix, long long rpix, float alpha,
-                                                  uint32_t stage, int team, int row, bool leader, int chunk_stride = 2,
-                                                  const EpiAux* aux = nullptr, uint32_t* sbuf = nullptr, int nbuf = 2) {
+                                                  uint32_t stage, int nbuf, uint32_t& sbuf, int team, int row, bool leader,
+                                                  const EpiAux* aux) {
+  static_assert(F == -1 || (F & (kEpiSmApply | kEpiSmBwd)) != 0, "other compile-time variants use epilogue_frag_chunk");
   constexpr int kTeamThreads = 128;
   constexpr bool sm_apply = F >= 0 && (F & kEpiSmApply) != 0, sm_bwd = F >= 0 && (F & kEpiSmBwd) != 0;
   constexpr float kLog2e = 1.4426950408889634f;
@@ -299,45 +360,26 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
     sm_a = -m * kLog2e; sm_b = 1.f / l;          // exponent offset in base-2 units
   }
   if (sm_bwd && valid) sm_a = __ldg(p.sm_delta + pix);
-  const bool has_bias = F < 0 ? p.bias != nullptr : (F & kEpiBias) != 0;
-  const bool do_relu = F < 0 ? p.relu != 0 : (F & kEpiRelu) != 0;
-  const bool res_pre = F < 0 ? (p.residual != nullptr && !p.res_after) : (F & kEpiResPre) != 0;
-  const bool res_post = F < 0 ? (p.residual != nullptr && p.res_after) : (F & kEpiResPost) != 0;
-  const bool has_mask = F < 0 ? (p.mask != nullptr || p.mask_bits != nullptr) : (F & kEpiMask) != 0;
-  const bool use_mbits = F < 0 ? (has_mask && p.mask_bits != nullptr) : (F & kEpiMaskBits) != 0;
-  const bool emit_bits = F < 0 ? (do_relu && p.relu_bits != nullptr) : (F & kEpiBitsOut) != 0;
-  // the ReLU is the last arithmetic of the piece (no mask, no post-mask residual): take the bits from the packed output words
-  constexpr bool bits_from_packed = F >= 0 && (F & kEpiBitsOut) != 0 && (F & (kEpiMask | kEpiResPost)) == 0;
+  const EpiOps<F> op(p);
   const long long nw = p.Cout >> 6;
-  const bool full_c = F >= 0 && (F & kEpiFull) != 0;       // no channel-tail tests
   const float rs = p.res_scale;
-  // sbuf != nullptr: the team owns ``nbuf`` (2..4) staging tiles used round-robin, so a chunk only waits for the store issued
-  // nbuf chunks ago -- the latency of the previous tensor stores is off the critical path and more bytes are in flight.
   const uint32_t sw = (uint32_t)(row & 7);
-  // 1: residual tile via TMA, 2: mask tile via TMA (compile-time for F >= 0: the host sets the aux bits iff it passes ``aux``)
-  const int aux_kind = F < 0 ? ((aux && (res_pre || res_post || has_mask)) ? aux->kind : 0)
-                             : ((F & kEpiAuxRes) ? 1 : ((F & kEpiAuxMask) ? 2 : (sm_bwd ? 3 : 0)));
+  // 1: residual tile via TMA, 2: mask tile via TMA, 3: the softmax backward's P tile
+  const int aux_kind = F >= 0 ? (sm_bwd ? 3 : 0) : (aux ? aux->kind : 0);
   const uint32_t asw = aux ? (uint32_t)(aux->arow & 7) : 0u;
-  for (int cc = (chunk_stride == 2 ? team : 0); cc * 64 < BN; cc += chunk_stride) {
+  for (int cc = team; cc * 64 < BN; cc += 2) {
     const int nbase = n0 + cc * 64;
     if (nbase >= p.Cout) break;
     uint32_t mlo = 0u, mhi = 0u, olo = 0u, ohi = 0u;
-    if (use_mbits && valid) {                    // 8 bytes instead of a 128-byte line of the bf16 activation
+    if (op.mask_bits && valid) {                 // 8 bytes instead of a 128-byte line of the bf16 activation
       const uint2 m = __ldg(reinterpret_cast<const uint2*>(p.mask_bits) + pix * nw + (nbase >> 6));
       mlo = m.x; mhi = m.y;
     }
-    const uint32_t stage_cur = stage + (sbuf ? *sbuf * kEpiStageBytes : 0u);
+    const uint32_t stage_cur = epi_stage_next(stage, kEpiStageBytes, nbuf, sbuf, leader);
     const uint32_t srow = stage_cur + (uint32_t)row * 128u;
-    if (leader) {                                // the store that last used this staging tile has finished reading it
-      if (!sbuf) bulk_wait_read0();
-      else if (nbuf == 2) bulk_wait_read1();
-      else if (nbuf == 3) bulk_wait_read2();
-      else bulk_wait_read3();
-    }
-    if (sbuf) *sbuf = (*sbuf + 1u == (uint32_t)nbuf) ? 0u : *sbuf + 1u;
     named_bar_sync(1 + team, kTeamThreads);
     uint32_t arow_addr = 0u, aslot = 0u;
-    if (aux_kind) {                              // residual / mask chunk: one TMA box (fetched ahead by the aux producer warp)
+    if (aux_kind) {                              // residual / mask / P chunk: one TMA box (fetched ahead by the aux producer warp)
       aslot = *aux->cnt % (uint32_t)aux->depth;
       mbar_wait(aux->full0 + 8u * aslot, (*aux->cnt / (uint32_t)aux->depth) & 1u);
       arow_addr = aux->ring + aslot * kEpiStageBytes + (uint32_t)aux->arow * 128u;
@@ -350,85 +392,46 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
         float f[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]) * alpha;
-        const int nvalid = full_c ? 16 : p.Cout - n;   // channels of this 16-wide piece inside the tensor: >= 16, 8 (Cout % 16 == 8) or <= 0
-        const bool in_c = full_c || nvalid > 0;
+        const int nvalid = op.full_c ? 16 : p.Cout - n;   // channels of this 16-wide piece inside the tensor: >= 16, 8 (Cout % 16 == 8) or <= 0
+        const bool in_c = op.full_c || nvalid > 0;
+        // 16 bf16 values of this row: this piece's two 16-byte units of the aux tile, or global memory (zero past the tensor)
+        auto load16 = [&](int kind, const bf16* src, uint32_t (&w)[8]) {
+#pragma unroll
+          for (int j = 0; j < 2; ++j)
+            reinterpret_cast<uint4*>(w)[j] = (aux_kind == kind) ? ld_shared_v4(arow_addr + (((uint32_t)(2 * s + j) ^ asw) << 4))
+                                             : ((op.full_c || 8 * j < nvalid) ? __ldg(reinterpret_cast<const uint4*>(src) + j)
+                                                                             : make_uint4(0u, 0u, 0u, 0u));
+        };
         if (sm_apply) {
 #pragma unroll
           for (int j = 0; j < 16; ++j) f[j] = fast_ex2(fmaf(f[j], kLog2e, sm_a)) * sm_b;
         }
         if (sm_bwd) {                                // dS = P * (dP - delta); P: this row of the aux tile
+          uint32_t pw[8];
+          load16(3, nullptr, pw);
 #pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const uint4 r = ld_shared_v4(arow_addr + (((uint32_t)(2 * s + j) ^ asw) << 4));
-            f[8 * j + 0] = bf16_bits_lo(r.x) * (f[8 * j + 0] - sm_a); f[8 * j + 1] = bf16_bits_hi(r.x) * (f[8 * j + 1] - sm_a);
-            f[8 * j + 2] = bf16_bits_lo(r.y) * (f[8 * j + 2] - sm_a); f[8 * j + 3] = bf16_bits_hi(r.y) * (f[8 * j + 3] - sm_a);
-            f[8 * j + 4] = bf16_bits_lo(r.z) * (f[8 * j + 4] - sm_a); f[8 * j + 5] = bf16_bits_hi(r.z) * (f[8 * j + 5] - sm_a);
-            f[8 * j + 6] = bf16_bits_lo(r.w) * (f[8 * j + 6] - sm_a); f[8 * j + 7] = bf16_bits_hi(r.w) * (f[8 * j + 7] - sm_a);
+          for (int k = 0; k < 8; ++k) {
+            f[2 * k] = bf16_bits_lo(pw[k]) * (f[2 * k] - sm_a); f[2 * k + 1] = bf16_bits_hi(pw[k]) * (f[2 * k + 1] - sm_a);
           }
         }
-        if (has_bias && in_c) {
-          const float4* bp = reinterpret_cast<const float4*>(p.bias + n);
+        float b[16] = {};
+        uint32_t r[8] = {}, m[8] = {}, w[8];
+        if (op.bias && in_c) {
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (full_c || 4 * j < nvalid) {
-              const float4 bb = __ldg(bp + j);
-              f[4 * j + 0] += bb.x; f[4 * j + 1] += bb.y; f[4 * j + 2] += bb.z; f[4 * j + 3] += bb.w;
-            }
-          }
+          for (int j = 0; j < 4; ++j)
+            if (op.full_c || 4 * j < nvalid) reinterpret_cast<float4*>(b)[j] = __ldg(reinterpret_cast<const float4*>(p.bias + n) + j);
         }
-        if (res_pre && in_c && valid) {
-          const uint4* rp = reinterpret_cast<const uint4*>(p.residual + rpix * p.res_cstride + n);
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const uint4 r = (aux_kind == 1) ? ld_shared_v4(arow_addr + (((uint32_t)(2 * s + j) ^ asw) << 4))
-                                            : ((full_c || 8 * j < nvalid) ? __ldg(rp + j) : make_uint4(0u, 0u, 0u, 0u));
-            f[8 * j + 0] = fmaf(bf16_bits_lo(r.x), rs, f[8 * j + 0]); f[8 * j + 1] = fmaf(bf16_bits_hi(r.x), rs, f[8 * j + 1]);
-            f[8 * j + 2] = fmaf(bf16_bits_lo(r.y), rs, f[8 * j + 2]); f[8 * j + 3] = fmaf(bf16_bits_hi(r.y), rs, f[8 * j + 3]);
-            f[8 * j + 4] = fmaf(bf16_bits_lo(r.z), rs, f[8 * j + 4]); f[8 * j + 5] = fmaf(bf16_bits_hi(r.z), rs, f[8 * j + 5]);
-            f[8 * j + 6] = fmaf(bf16_bits_lo(r.w), rs, f[8 * j + 6]); f[8 * j + 7] = fmaf(bf16_bits_hi(r.w), rs, f[8 * j + 7]);
-          }
-        }
+        if ((op.res_pre || op.res_post) && in_c && valid) load16(1, p.residual + rpix * p.res_cstride + n, r);
+        if (op.mask && !op.mask_bits && in_c && valid) load16(2, p.mask + pix * p.mask_cstride + n, m);
         uint32_t ob = 0u;
-        if (do_relu) {
 #pragma unroll
-          for (int j = 0; j < 16; ++j) f[j] = fmaxf(f[j], 0.f);
-          if (emit_bits && !bits_from_packed) ob = positive_bits16(f);
-        }
-        if (use_mbits) {
-          apply_bits16(f, mb);
-        } else if (has_mask && in_c && valid) {
-          const uint4* mp = reinterpret_cast<const uint4*>(p.mask + pix * p.mask_cstride + n);
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const uint4 m = (aux_kind == 2) ? ld_shared_v4(arow_addr + (((uint32_t)(2 * s + j) ^ asw) << 4))
-                                            : ((full_c || 8 * j < nvalid) ? __ldg(mp + j) : make_uint4(0u, 0u, 0u, 0u));
-            f[8 * j + 0] = bf16_bits_lo(m.x) > 0.f ? f[8 * j + 0] : 0.f;
-            f[8 * j + 1] = bf16_bits_hi(m.x) > 0.f ? f[8 * j + 1] : 0.f;
-            f[8 * j + 2] = bf16_bits_lo(m.y) > 0.f ? f[8 * j + 2] : 0.f;
-            f[8 * j + 3] = bf16_bits_hi(m.y) > 0.f ? f[8 * j + 3] : 0.f;
-            f[8 * j + 4] = bf16_bits_lo(m.z) > 0.f ? f[8 * j + 4] : 0.f;
-            f[8 * j + 5] = bf16_bits_hi(m.z) > 0.f ? f[8 * j + 5] : 0.f;
-            f[8 * j + 6] = bf16_bits_lo(m.w) > 0.f ? f[8 * j + 6] : 0.f;
-            f[8 * j + 7] = bf16_bits_hi(m.w) > 0.f ? f[8 * j + 7] : 0.f;
-          }
-        }
-        if (res_post && in_c && valid) {
-          const uint4* rp = reinterpret_cast<const uint4*>(p.residual + rpix * p.res_cstride + n);
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const uint4 r = (aux_kind == 1) ? ld_shared_v4(arow_addr + (((uint32_t)(2 * s + j) ^ asw) << 4))
-                                            : ((full_c || 8 * j < nvalid) ? __ldg(rp + j) : make_uint4(0u, 0u, 0u, 0u));
-            f[8 * j + 0] = fmaf(bf16_bits_lo(r.x), rs, f[8 * j + 0]); f[8 * j + 1] = fmaf(bf16_bits_hi(r.x), rs, f[8 * j + 1]);
-            f[8 * j + 2] = fmaf(bf16_bits_lo(r.y), rs, f[8 * j + 2]); f[8 * j + 3] = fmaf(bf16_bits_hi(r.y), rs, f[8 * j + 3]);
-            f[8 * j + 4] = fmaf(bf16_bits_lo(r.z), rs, f[8 * j + 4]); f[8 * j + 5] = fmaf(bf16_bits_hi(r.z), rs, f[8 * j + 5]);
-            f[8 * j + 6] = fmaf(bf16_bits_lo(r.w), rs, f[8 * j + 6]); f[8 * j + 7] = fmaf(bf16_bits_hi(r.w), rs, f[8 * j + 7]);
-          }
+        for (int k = 0; k < 8; ++k) {
+          uint32_t pos;
+          const float2 o = epi_pair(op, f[2 * k], f[2 * k + 1], make_float2(b[2 * k], b[2 * k + 1]), r[k], m[k], mb >> (2 * k), rs, pos);
+          ob |= pos << (2 * k);
+          w[k] = pack_bf16x2(o.x, o.y);
         }
         // 16 channels = two 16-byte units (2s, 2s+1) of this row's 128-byte line; unit u lives at (u ^ (row & 7))
-        uint32_t w[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) w[j] = pack_bf16x2(f[2 * j], f[2 * j + 1]);
-        if (bits_from_packed) ob = positive_bits16_packed(w);
         st_shared_v4(srow + (((uint32_t)(2 * s) ^ sw) << 4), w[0], w[1], w[2], w[3]);
         st_shared_v4(srow + (((uint32_t)(2 * s + 1) ^ sw) << 4), w[4], w[5], w[6], w[7]);
         return ob;
@@ -446,7 +449,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
         else ohi |= ob << (16 * (s & 1));
       }
     }
-    if (emit_bits && valid) {
+    if (op.bits_out && valid) {
       reinterpret_cast<uint2*>(p.relu_bits)[pix * nw + (nbase >> 6)] = make_uint2(olo, ohi);
     }
     fence_proxy_async_smem();                    // generic-proxy smem writes -> visible to the TMA (async proxy)
@@ -462,11 +465,9 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
 // -------------------------------------------------------------------------------------------------------------------
 // Epilogue straight from the wgmma accumulator registers of one warpgroup: 64 pixel rows x BN channels in the Wgmma
 // fragment layout (thread = warp w, lane l of the warpgroup: rows 16w + l/4 and 16w + l/4 + 8, columns 8j + 2(l%4) + 0 / 1).
-// No fp32 staging: per 64-channel chunk the warpgroup packs bf16 pairs into a SWIZZLE_128B staging tile [64 rows][64 ch]
-// (8 KiB; a thread's pair of column block j goes to 16-byte unit j ^ (row & 7), conflict-free) and one thread issues the
-// TMA store of the box (64 ch, 64 px).  Per element the arithmetic is that of epilogue_tile_tma's piece(): acc * alpha,
-// + bias, fmaf(residual, rs, .), ReLU, mask, fmaf(post-mask residual, rs, .), bf16 pack -- the outputs are bit-identical.
-// ReLU bit planes are OR-reduced over the four lanes that share a row.
+// No fp32 staging: per 64-channel chunk the warpgroup packs bf16 pairs (epi_pair) into a SWIZZLE_128B staging tile
+// [64 rows][64 ch] (8 KiB; a thread's pair of column block j goes to 16-byte unit j ^ (row & 7), conflict-free) and one thread
+// issues the TMA store of the box (64 ch, 64 px).  ReLU bit planes are OR-reduced over the four lanes that share a row.
 //   cc         : 64-channel chunk of the accumulator (compile-time after unrolling: the fragments stay in registers).
 //   pix / rpix : output / residual pixel of this thread's two rows; valid: the row lies inside the output (rows outside are
 //                clipped by the TMA store; their global loads read pixel 0 and their bit-plane words are not written).
@@ -484,32 +485,21 @@ __device__ __forceinline__ void epilogue_frag_chunk(const EpiArgs& p, const CUte
                                                     const uint32_t (&arow)[2] = {0u, 0u}) {
   static_assert(F < 0 || (F & (kEpiSmStats | kEpiSmApply | kEpiSmBwd)) == 0, "softmax epilogues are served by epilogue_tile_tma");
   constexpr int aux_kind = F < 0 ? 0 : ((F & kEpiAuxRes) ? 1 : ((F & kEpiAuxMask) ? 2 : 0));
-  const bool has_bias = F < 0 ? p.bias != nullptr : (F & kEpiBias) != 0;
-  const bool do_relu = F < 0 ? p.relu != 0 : (F & kEpiRelu) != 0;
-  const bool res_pre = F < 0 ? (p.residual != nullptr && !p.res_after) : (F & kEpiResPre) != 0;
-  const bool res_post = F < 0 ? (p.residual != nullptr && p.res_after) : (F & kEpiResPost) != 0;
-  const bool has_mask = F < 0 ? (p.mask != nullptr || p.mask_bits != nullptr) : (F & kEpiMask) != 0;
-  const bool use_mbits = F < 0 ? (has_mask && p.mask_bits != nullptr) : (F & kEpiMaskBits) != 0;
-  const bool emit_bits = F < 0 ? (do_relu && p.relu_bits != nullptr) : (F & kEpiBitsOut) != 0;
+  // the ReLU is the last arithmetic of the pair (no mask, no post-mask residual): take the bits from the packed output word --
+  // adding 0x7FFF to a post-ReLU bf16 half (+0 or a positive value <= 0x7F80) sets its bit 15 iff it is non-zero, without
+  // carrying into its neighbour; fewer instructions than a compare per element, and the bit plane is paid for by write-bound layers
   constexpr bool bits_from_packed = F >= 0 && (F & kEpiBitsOut) != 0 && (F & (kEpiMask | kEpiResPost)) == 0;
-  const bool full_c = F >= 0 && (F & kEpiFull) != 0;
+  const EpiOps<F> op(p);
   const float rs = p.res_scale;
   const long long nw = p.Cout >> 6;
   const uint32_t w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31, q = l & 3;
   const uint32_t r0 = 16u * w + (l >> 2);
   const long long lpix[2] = {valid[0] ? pix[0] : 0ll, valid[1] ? pix[1] : 0ll};
   const long long lrpix[2] = {valid[0] ? rpix[0] : 0ll, valid[1] ? rpix[1] : 0ll};
-  const uint32_t stage_cur = stage + sbuf * kFragStageBytes;
-  if (leader) {                                  // the store that last used this staging tile has finished reading it
-    if (nbuf == 1) bulk_wait_read0();
-    else if (nbuf == 2) bulk_wait_read1();
-    else if (nbuf == 3) bulk_wait_read2();
-    else bulk_wait_read3();
-  }
-  sbuf = (sbuf + 1u == (uint32_t)nbuf) ? 0u : sbuf + 1u;
+  const uint32_t stage_cur = epi_stage_next(stage, kFragStageBytes, nbuf, sbuf, leader);
   named_bar_sync(bar, 128);
   uint32_t mb[2][2] = {{0u, 0u}, {0u, 0u}}, ob[2][2] = {{0u, 0u}, {0u, 0u}};
-  if (use_mbits) {
+  if (op.mask_bits) {
 #pragma unroll
     for (int hr = 0; hr < 2; ++hr) {
       const uint2 m = __ldg(reinterpret_cast<const uint2*>(p.mask_bits) + lpix[hr] * nw + (nbase >> 6));
@@ -520,48 +510,34 @@ __device__ __forceinline__ void epilogue_frag_chunk(const EpiArgs& p, const CUte
   for (int jj = 0; jj < 8; ++jj) {
     const int j = cc * 8 + jj;                   // 8-column block of the accumulator
     const int n = nbase + 8 * jj + 2 * (int)q;
-    const bool in_c = full_c || nbase + 8 * jj < p.Cout;      // Cout % 8 == 0: a column block is all in or all out
+    const bool in_c = op.full_c || nbase + 8 * jj < p.Cout;   // Cout % 8 == 0: a column block is all in or all out
     const uint32_t bit = 8u * (jj & 3) + 2u * q;              // bit of column 0 of the pair in its 32-bit half of the word
     float2 bb = make_float2(0.f, 0.f);
-    if (has_bias && in_c) bb = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+    if (op.bias && in_c) bb = __ldg(reinterpret_cast<const float2*>(p.bias + n));
 #pragma unroll
     for (int hr = 0; hr < 2; ++hr) {
       // this pair's 4 bytes in the aux box: 16-byte unit jj of row arow sits at jj ^ (arow & 7), conflict-free like the staging
       const uint32_t aaddr = aux_tile + arow[hr] * 128u + ((((uint32_t)jj) ^ (arow[hr] & 7u)) << 4) + 4u * q;
-      float f0 = acc[4 * j + 2 * hr] * alpha, f1 = acc[4 * j + 2 * hr + 1] * alpha;
-      if (has_bias && in_c) { f0 += bb.x; f1 += bb.y; }
-      if (res_pre && in_c) {
-        const uint32_t r = aux_kind == 1 ? ld_shared_b32(aaddr)
-                                         : __ldg(reinterpret_cast<const unsigned int*>(p.residual + lrpix[hr] * p.res_cstride + n));
-        f0 = fmaf(bf16_bits_lo(r), rs, f0); f1 = fmaf(bf16_bits_hi(r), rs, f1);
-      }
-      if (do_relu) {
-        f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f);
-        if (emit_bits && !bits_from_packed) ob[hr][jj >> 2] |= ((f0 > 0.f) ? 1u : 0u) << bit | ((f1 > 0.f) ? 1u : 0u) << (bit + 1);
-      }
-      if (use_mbits) {
-        const uint32_t m = mb[hr][jj >> 2] >> bit;
-        f0 = (m & 1u) ? f0 : 0.f; f1 = (m & 2u) ? f1 : 0.f;
-      } else if (has_mask && in_c) {
-        const uint32_t m = aux_kind == 2 ? ld_shared_b32(aaddr)
-                                         : __ldg(reinterpret_cast<const unsigned int*>(p.mask + lpix[hr] * p.mask_cstride + n));
-        f0 = bf16_bits_lo(m) > 0.f ? f0 : 0.f; f1 = bf16_bits_hi(m) > 0.f ? f1 : 0.f;
-      }
-      if (res_post && in_c) {
-        const uint32_t r = aux_kind == 1 ? ld_shared_b32(aaddr)
-                                         : __ldg(reinterpret_cast<const unsigned int*>(p.residual + lrpix[hr] * p.res_cstride + n));
-        f0 = fmaf(bf16_bits_lo(r), rs, f0); f1 = fmaf(bf16_bits_hi(r), rs, f1);
-      }
-      const uint32_t pk = pack_bf16x2(f0, f1);
-      if (bits_from_packed) {                    // as positive_bits16_packed: a half is flagged iff it is not +0
+      uint32_t res = 0u, msk = 0u, pos;
+      if ((op.res_pre || op.res_post) && in_c)
+        res = aux_kind == 1 ? ld_shared_b32(aaddr)
+                            : __ldg(reinterpret_cast<const unsigned int*>(p.residual + lrpix[hr] * p.res_cstride + n));
+      if (op.mask && !op.mask_bits && in_c)
+        msk = aux_kind == 2 ? ld_shared_b32(aaddr) : __ldg(reinterpret_cast<const unsigned int*>(p.mask + lpix[hr] * p.mask_cstride + n));
+      const float2 o = epi_pair(op, acc[4 * j + 2 * hr] * alpha, acc[4 * j + 2 * hr + 1] * alpha, bb, res, msk,
+                                mb[hr][jj >> 2] >> bit, rs, pos);
+      const uint32_t pk = pack_bf16x2(o.x, o.y);
+      if (bits_from_packed) {
         const uint32_t t = pk + 0x7FFF7FFFu;
         ob[hr][jj >> 2] |= ((t >> 15) & 1u) << bit | (t >> 31) << (bit + 1);
+      } else if (op.bits_out) {
+        ob[hr][jj >> 2] |= pos << bit;
       }
       const uint32_t r = r0 + 8u * hr;
       st_shared_b32(stage_cur + r * 128u + ((((uint32_t)jj) ^ (r & 7u)) << 4) + 4u * q, pk);
     }
   }
-  if (emit_bits) {
+  if (op.bits_out) {
 #pragma unroll
     for (int hr = 0; hr < 2; ++hr) {
 #pragma unroll

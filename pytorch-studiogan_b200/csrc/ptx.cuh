@@ -12,8 +12,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
-
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
@@ -56,12 +54,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
 }
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
@@ -82,10 +74,14 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src,
                : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read2() { asm volatile("cp.async.bulk.wait_group.read 2;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read3() { asm volatile("cp.async.bulk.wait_group.read 3;" ::: "memory"); }
+// Waits until the oldest of the last n (1..4) committed bulk groups has finished reading its shared-memory source: at most
+// n - 1 groups are still reading.
+__device__ __forceinline__ void bulk_wait_read(int n) {
+  if (n == 1) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+  else if (n == 2) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
+  else if (n == 3) asm volatile("cp.async.bulk.wait_group.read 2;" ::: "memory");
+  else asm volatile("cp.async.bulk.wait_group.read 3;" ::: "memory");
+}
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -184,8 +180,9 @@ __device__ __forceinline__ void acc_fence(float (&d)[R]) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// Accumulator staging in shared memory: fp32 rows of ``ld`` bytes, 16 more than the row (the padding staggers consecutive
-// rows across the banks, so the one-row-per-thread 16-byte reads of the fused epilogues do not conflict).
+// Accumulator staging in shared memory: fp32 rows of ``ld`` = acc_row_bytes(N) bytes, 16 more than the row (the padding
+// staggers consecutive rows across the banks, so the one-row-per-thread 16-byte reads of the fused epilogues do not conflict).
+__host__ __device__ inline uint32_t acc_row_bytes(int N) { return (uint32_t)N * 4u + 16u; }
 // Stores this warpgroup's 64-row fragment at ``base`` (its first row).
 template <int N>
 __device__ __forceinline__ void acc_store(const float (&d)[N / 2], uint32_t base, uint32_t ld) {

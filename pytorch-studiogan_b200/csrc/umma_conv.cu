@@ -32,9 +32,6 @@ static constexpr int kBlockK = 64;          // bf16 elements per 128-byte swizzl
 static constexpr int kABytes = kTileM * kBlockK * 2;  // 16 KiB
 static constexpr uint32_t kAccBar = 3;      // named barrier of the 256 consumer threads (1, 2: epilogue teams)
 
-// fp32 accumulator staging rows: BN columns + 16 bytes of padding (see acc_store)
-__host__ __device__ inline uint32_t acc_row_bytes(int BN) { return (uint32_t)BN * 4u + 16u; }
-
 struct FpropArgs {
   int B, H, W, Cin, Cout, taps, KW, pad_h, pad_w;
   int tw, th, nb;                 // tile box: tw*th*nb == 128
@@ -52,63 +49,24 @@ struct FpropArgs {
   EpiArgs e;
 };
 
-// Main loop of one fprop tile for this consumer warpgroup (rows 64 wg .. 64 wg + 63), then its accumulators -> shared memory.
-template <int BN>
-__device__ __forceinline__ void fprop_mma_tile(const FpropArgs& p, uint32_t smem_base, uint32_t stage_bytes, uint32_t bres_base,
-                                               uint32_t b_bytes, uint32_t bar_base, uint32_t& it, int wg, uint32_t acc_base) {
-  float acc[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  const bool b_mn = (p.w_mode == 2);
-  const int kiters = p.taps * p.kblocks;
-  const uint32_t lane = threadIdx.x & 31;
-  int prev = -1;
-  for (int k = 0; k < kiters; ++k, ++it) {
-    const int s = it % p.stages;
-    const uint32_t ph = (it / p.stages) & 1;
-    mbar_wait(bar_base + 8u * s, ph);
-    const uint32_t sa = smem_base + s * stage_bytes;
-    const uint64_t adesc = make_sdesc_sw128(sa + (uint32_t)wg * 8192u, 16, 1024);   // rows 64 wg.. of [128][64]
-    // K-major B: rows = output channels, +32 B per 16-wide K step.
-    // MN-major B: (BN/64) atoms of [64 k-rows][64 n] 8 KiB apart (LBO), 8-row groups 1 KiB apart (SBO), +2 KiB per K step.
-    const uint32_t sb = p.b_resident ? bres_base + (uint32_t)k * b_bytes : sa + kABytes;     // k = tap * kblocks + kb
-    wgmma_fence();
-    if (b_mn) {
-      const uint64_t bdesc = make_sdesc_sw128(sb, 8192, 1024);
-#pragma unroll
-      for (int kk = 0; kk < kBlockK / 16; ++kk) Wgmma<BN>::template mma<0, 1>(acc, adesc + 2 * kk, bdesc + 128 * kk, (k > 0 || kk > 0) ? 1u : 0u);
-    } else {
-      const uint64_t bdesc = make_sdesc_sw128(sb, 16, 1024);
-#pragma unroll
-      for (int kk = 0; kk < kBlockK / 16; ++kk) Wgmma<BN>::template mma<0, 0>(acc, adesc + 2 * kk, bdesc + 2 * kk, (k > 0 || kk > 0) ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<1>();                          // the previous K block's MMAs have retired: its ring slot is free
-    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev)); }
-    prev = s;
-  }
-  wgmma_wait<0>();
-  acc_fence(acc);
-  __syncwarp();
-  if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev));
-  named_bar_sync(kAccBar, kConsumerThreads);  // every consumer is done reading the previous tile's staged accumulators
-  acc_store<BN>(acc, acc_base + (uint32_t)wg * 64u * acc_row_bytes(BN), acc_row_bytes(BN));
-  named_bar_sync(kAccBar, kConsumerThreads);
+// Tile index -> (channel tile, w / h / batch tile of the (tw, th, nb) box), channel tiles fastest.
+struct FpropTile { int nt, wt, ht, bt; };
+__device__ __forceinline__ FpropTile fprop_tile(const FpropArgs& p, int t) {
+  FpropTile c;
+  c.nt = t % p.tiles_n; t /= p.tiles_n;
+  c.wt = t % p.tiles_w; t /= p.tiles_w;
+  c.ht = t % p.tiles_h; t /= p.tiles_h;
+  c.bt = t;
+  return c;
 }
 
-// ------------------------------------------------------------------------------------------------ fprop, ping-pong schedule
-// Compile-time epilogue variants other than the softmax ones: each consumer warpgroup owns whole 128-row tiles (local tile i
-// goes to warpgroup i & 1) and runs the epilogue straight from its registers while the other warpgroup issues its MMAs.
-__host__ __device__ constexpr bool fprop_is_pingpong(int f) { return f >= 0 && (f & (kEpiSmStats | kEpiSmApply | kEpiSmBwd)) == 0; }
-static constexpr uint32_t kTurnBar = 4;       // named barriers 4 / 5: warpgroup 0 / 1 may start its next mainloop
-
-// Main loop of one 128-row tile on one warpgroup: per 16-wide K step two m64 wgmmas (rows 0..63 -> acc[0], 64..127 -> acc[1])
-// against the same B tile.  it = the tile's first position in the operand ring.
-template <int BN>
-__device__ __forceinline__ void fprop_pp_mma(const FpropArgs& p, float (&acc)[2][BN / 2], uint32_t smem_base, uint32_t stage_bytes,
-                                             uint32_t bres_base, uint32_t b_bytes, uint32_t bar_base, uint32_t it) {
+// Main loop of one fprop tile on one consumer warpgroup: per 16-wide K step, M m64 wgmmas against the same B tile, row block h
+// of the A tile at a_off + h * 8 KiB -> acc[h].  it = the tile's first position in the operand ring.
+template <int BN, int M>
+__device__ __forceinline__ void fprop_mma(const FpropArgs& p, float (&acc)[M][BN / 2], uint32_t a_off, uint32_t smem_base,
+                                          uint32_t stage_bytes, uint32_t bres_base, uint32_t b_bytes, uint32_t bar_base, uint32_t it) {
 #pragma unroll
-  for (int h = 0; h < 2; ++h)
+  for (int h = 0; h < M; ++h)
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
   const bool b_mn = (p.w_mode == 2);
@@ -120,22 +78,24 @@ __device__ __forceinline__ void fprop_pp_mma(const FpropArgs& p, float (&acc)[2]
     const uint32_t ph = (it / p.stages) & 1;
     mbar_wait(bar_base + 8u * s, ph);
     const uint32_t sa = smem_base + s * stage_bytes;
-    const uint64_t adesc = make_sdesc_sw128(sa, 16, 1024);                 // [128][64]; rows 64.. are 8 KiB further
-    const uint32_t sb = p.b_resident ? bres_base + (uint32_t)k * b_bytes : sa + kABytes;
+    const uint64_t adesc = make_sdesc_sw128(sa + a_off, 16, 1024);          // [128][64]; row block h is 8 KiB further
+    // K-major B: rows = output channels, +32 B per 16-wide K step.
+    // MN-major B: (BN/64) atoms of [64 k-rows][64 n] 8 KiB apart (LBO), 8-row groups 1 KiB apart (SBO), +2 KiB per K step.
+    const uint32_t sb = p.b_resident ? bres_base + (uint32_t)k * b_bytes : sa + kABytes;     // k = tap * kblocks + kb
     wgmma_fence();
     if (b_mn) {
       const uint64_t bdesc = make_sdesc_sw128(sb, 8192, 1024);
 #pragma unroll
       for (int kk = 0; kk < kBlockK / 16; ++kk)
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
+        for (int h = 0; h < M; ++h)
           Wgmma<BN>::template mma<0, 1>(acc[h], adesc + 512 * h + 2 * kk, bdesc + 128 * kk, (k > 0 || kk > 0) ? 1u : 0u);
     } else {
       const uint64_t bdesc = make_sdesc_sw128(sb, 16, 1024);
 #pragma unroll
       for (int kk = 0; kk < kBlockK / 16; ++kk)
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
+        for (int h = 0; h < M; ++h)
           Wgmma<BN>::template mma<0, 0>(acc[h], adesc + 512 * h + 2 * kk, bdesc + 2 * kk, (k > 0 || kk > 0) ? 1u : 0u);
     }
     wgmma_commit();
@@ -144,11 +104,29 @@ __device__ __forceinline__ void fprop_pp_mma(const FpropArgs& p, float (&acc)[2]
     prev = s;
   }
   wgmma_wait<0>();
-  acc_fence(acc[0]);
-  acc_fence(acc[1]);
+#pragma unroll
+  for (int h = 0; h < M; ++h) acc_fence(acc[h]);
   __syncwarp();
   if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev));
 }
+
+// Staged schedule: the main loop of this consumer warpgroup's 64 rows (64 wg .. 64 wg + 63) of the tile, then its accumulators
+// -> shared memory.
+template <int BN>
+__device__ __forceinline__ void fprop_staged_mma(const FpropArgs& p, uint32_t smem_base, uint32_t stage_bytes, uint32_t bres_base,
+                                                 uint32_t b_bytes, uint32_t bar_base, uint32_t it, int wg, uint32_t acc_base) {
+  float acc[1][BN / 2];
+  fprop_mma<BN, 1>(p, acc, (uint32_t)wg * 8192u, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it);
+  named_bar_sync(kAccBar, kConsumerThreads);  // every consumer is done reading the previous tile's staged accumulators
+  acc_store<BN>(acc[0], acc_base + (uint32_t)wg * 64u * acc_row_bytes(BN), acc_row_bytes(BN));
+  named_bar_sync(kAccBar, kConsumerThreads);
+}
+
+// ------------------------------------------------------------------------------------------------ fprop, ping-pong schedule
+// Compile-time epilogue variants other than the softmax ones: each consumer warpgroup owns whole 128-row tiles (local tile i
+// goes to warpgroup i & 1) and runs the epilogue straight from its registers while the other warpgroup issues its MMAs.
+__host__ __device__ constexpr bool fprop_is_pingpong(int f) { return f >= 0 && (f & (kEpiSmStats | kEpiSmApply | kEpiSmBwd)) == 0; }
+static constexpr uint32_t kTurnBar = 4;       // named barriers 4 / 5: warpgroup 0 / 1 may start its next mainloop
 
 // One consumer warpgroup of the ping-pong schedule.  The two warpgroups' main loops take turns (named barriers kTurnBar + wg),
 // so warpgroup A's epilogue runs under warpgroup B's MMAs.  The epilogue stores the tile as two 64-row half boxes per
@@ -161,7 +139,7 @@ __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUte
   constexpr int aux_kind = (F & kEpiAuxRes) ? 1 : ((F & kEpiAuxMask) ? 2 : 0);
   const uint32_t w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const bool leader = (threadIdx.x & 127) == 0;
-  const float alpha = p.e.alpha_ptr ? p.e.alpha * __ldg(p.e.alpha_ptr) : p.e.alpha;
+  const float alpha = epi_alpha(p.e);
   // the half box splits the outermost non-unit dimension of (tw, th, nb): 0 = w, 1 = h, 2 = b
   const int split = p.nb > 1 ? 2 : (p.th > 1 ? 1 : 0);
   // tile coordinates and aux-box row of this thread's four rows: half h, fragment row hr -> tile row 64 h + 16 w + lane / 4 + 8 hr
@@ -186,14 +164,11 @@ __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUte
   uint32_t sbuf = 0, aux_cnt = 0;
   if (p.b_resident) mbar_wait(bar_base + 8u * (2 * p.stages), 0);
   for (int i = wg; i < n_local; i += 2) {
-    int t = (int)blockIdx.x + i * (int)gridDim.x;
-    const int nt = t % p.tiles_n; t /= p.tiles_n;
-    const int wt = t % p.tiles_w; t /= p.tiles_w;
-    const int ht = t % p.tiles_h; t /= p.tiles_h;
-    const int bt = t;
+    const FpropTile tc = fprop_tile(p, (int)blockIdx.x + i * (int)gridDim.x);
+    const int nt = tc.nt, wt = tc.wt, ht = tc.ht, bt = tc.bt;
     float acc[2][BN / 2];
     if (i > 0) named_bar_sync(kTurnBar + wg, 256);          // the other warpgroup has issued tile i - 1
-    fprop_pp_mma<BN>(p, acc, smem_base, stage_bytes, bres_base, b_bytes, bar_base, (uint32_t)(i * kiters));
+    fprop_mma<BN, 2>(p, acc, 0u, smem_base, stage_bytes, bres_base, b_bytes, bar_base, (uint32_t)(i * kiters));
     if (i + 1 < n_local) named_bar_arrive(kTurnBar + (wg ^ 1), 256);
     long long pix[2][2], rpix[2][2];
     bool valid[2][2];
@@ -208,7 +183,7 @@ __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUte
         const int x = wt * p.tw + wi[h][hr], y = ht * p.th + hi[h][hr], b = bt * p.nb + bi[h][hr];
         valid[h][hr] = x < p.W && y < p.H && b < p.B;
         pix[h][hr] = ((long long)b * p.H + y) * p.W + x;
-        rpix[h][hr] = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (y >> 1)) * (p.W >> 1) + (x >> 1)) : pix[h][hr];
+        rpix[h][hr] = epi_rpix(p.e, b, y, x, p.H, p.W, pix[h][hr]);
       }
     }
 #pragma unroll                                    // static accumulator indices: the fragments stay in registers
@@ -248,9 +223,10 @@ __device__ __forceinline__ void fprop_staged_consumer(const FpropArgs& p, const 
   const bool leader = (q == 0) && (lane == 0);
   const int wi = row % p.tw, hi = (row / p.tw) % p.th, bi = row / (p.tw * p.th);
   const bool vec_ok = epi_vec_ok(p.e);
-  const float alpha = p.e.alpha_ptr ? p.e.alpha * __ldg(p.e.alpha_ptr) : p.e.alpha;
+  const float alpha = epi_alpha(p.e);
   const uint32_t stage = epi_stage_base + team * p.epi_nbuf * kEpiStageBytes;
   const uint32_t t_row = acc_base + (uint32_t)row * acc_row_bytes(p.BN);
+  const int kiters = p.taps * p.kblocks;
   uint32_t aux_cnt = 0, sbuf = 0, it = 0;
   EpiAux aux;
   aux.kind = p.aux_kind; aux.ring = aux_stage_base + (uint32_t)(team * p.aux_depth) * kEpiStageBytes;
@@ -260,30 +236,27 @@ __device__ __forceinline__ void fprop_staged_consumer(const FpropArgs& p, const 
   const bool aux_half = p.aux_kind == 1 && p.e.res_up2;
   aux.arow = aux_half ? ((bi * p.aux_th + (p.aux_th == p.th ? hi : (hi >> 1))) * p.aux_tw + (wi >> 1)) : row;
   if (p.b_resident) mbar_wait(bar_base + 8u * (2 * p.stages), 0);
-  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-    int t = tile;
-    const int nt = t % p.tiles_n; t /= p.tiles_n;
-    const int wt = t % p.tiles_w; t /= p.tiles_w;
-    const int ht = t % p.tiles_h; t /= p.tiles_h;
-    const int bt = t;
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, it += kiters) {
+    const FpropTile tc = fprop_tile(p, tile);
+    const int nt = tc.nt, wt = tc.wt, ht = tc.ht, bt = tc.bt;
     const int n0 = nt * p.BN;
     const int w = wt * p.tw + wi, h = ht * p.th + hi, b = bt * p.nb + bi;
     const bool valid = (w < p.W) && (h < p.H) && (b < p.B) && (p.out_sub == 1 || (((w | h) & 1) == 0));
     const long long pix = p.out_sub == 1 ? ((long long)b * p.H + h) * p.W + w
                                          : ((long long)b * ((p.H + 1) >> 1) + (h >> 1)) * ((p.W + 1) >> 1) + (w >> 1);
-    const long long rpix = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1)) : pix;
+    const long long rpix = epi_rpix(p.e, b, h, w, p.H, p.W, pix);
 
     switch (p.BN) {
-      case 16: fprop_mma_tile<16>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
-      case 32: fprop_mma_tile<32>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
-      case 64: fprop_mma_tile<64>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
-      default: fprop_mma_tile<128>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+      case 16: fprop_staged_mma<16>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+      case 32: fprop_staged_mma<32>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+      case 64: fprop_staged_mma<64>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+      default: fprop_staged_mma<128>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
     }
     if constexpr (F >= 0 && (F & kEpiSmStats) != 0) {
       epilogue_tile_smstats(p.e, t_row, p.BN, n0, valid, pix, alpha, team, nt * 2 + team);
     } else if (p.use_tma) {
-      epilogue_tile_tma<F>(p.e, tmY, t_row, p.BN, n0, wt * p.tw, ht * p.th, bt * p.nb, valid, pix, rpix, alpha, stage, team, row,
-                           leader, 2, p.aux_kind ? &aux : nullptr, p.epi_nbuf >= 2 ? &sbuf : nullptr, p.epi_nbuf);
+      epilogue_tile_tma<F>(p.e, tmY, t_row, p.BN, n0, wt * p.tw, ht * p.th, bt * p.nb, valid, pix, rpix, alpha, stage, p.epi_nbuf,
+                           sbuf, team, row, leader, p.aux_kind ? &aux : nullptr);
     } else if (team == 0) {
       epilogue_row(p.e, t_row, p.BN, n0, valid, pix, rpix, alpha, vec_ok);
     }
@@ -354,12 +327,8 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             tma_load_3d(bres_base + (uint32_t)(tap * p.kblocks + kb) * b_bytes, &tmB, bres_bar, kb * kBlockK, tap, 0);
       }
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        int t = tile;
-        const int nt = t % p.tiles_n; t /= p.tiles_n;
-        const int wt = t % p.tiles_w; t /= p.tiles_w;
-        const int ht = t % p.tiles_h; t /= p.tiles_h;
-        const int bt = t;
-        const int n0 = nt * p.BN, w0 = wt * p.tw, h0 = ht * p.th, b0 = bt * p.nb;
+        const FpropTile tc = fprop_tile(p, tile);
+        const int n0 = tc.nt * p.BN, w0 = tc.wt * p.tw, h0 = tc.ht * p.th, b0 = tc.bt * p.nb;
         for (int tap = 0; tap < p.taps; ++tap) {
           const int dh = tap / p.KW - p.pad_h, dw = tap % p.KW - p.pad_w;
           for (int kb = 0; kb < p.kblocks; ++kb, ++it) {
@@ -391,13 +360,10 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const uint32_t bytes = (uint32_t)(p.aux_tw * p.aux_th * p.nb) * 128u;
       uint32_t cnt[2] = {0u, 0u};
       for (int tile = blockIdx.x, i = 0; tile < p.num_tiles; tile += gridDim.x, ++i) {
-        int t = tile;
-        const int nt = t % p.tiles_n; t /= p.tiles_n;
-        const int wt = t % p.tiles_w; t /= p.tiles_w;
-        const int ht = t % p.tiles_h; t /= p.tiles_h;
-        const int c1 = half ? (wt * p.tw) >> 1 : wt * p.tw, c2 = half ? (ht * p.th) >> 1 : ht * p.th, c3 = t * p.nb;
+        const FpropTile tc = fprop_tile(p, tile);
+        const int c1 = half ? (tc.wt * p.tw) >> 1 : tc.wt * p.tw, c2 = half ? (tc.ht * p.th) >> 1 : tc.ht * p.th, c3 = tc.bt * p.nb;
         for (int cc = 0; cc * 64 < p.BN; ++cc) {
-          const int nbase = nt * p.BN + cc * 64;
+          const int nbase = tc.nt * p.BN + cc * 64;
           if (nbase >= p.e.Cout) break;
           const int team = pingpong ? (i & 1) : (cc & 1);
           const uint32_t slot = cnt[team] % (uint32_t)p.aux_depth;
@@ -583,8 +549,15 @@ static void pick_tile(int H, int W, int B, int& tw, int& th, int& nb) {
   (void)B;
 }
 
+// The epilogue can stage bf16 64-channel chunks and TMA-store them: a bf16 output, channel tiles of 64, 16-byte aligned
+// channel strides of every tensor it reads or writes.
+bool epi_tma_ok(const sgb_conv_desc* d, int BN) {
+  return !d->y_fp32 && BN % 64 == 0 && d->Cout % 8 == 0 && d->y_cstride % 8 == 0 && (!d->residual || d->res_cstride % 8 == 0) &&
+         (!d->mask || d->mask_cstride % 8 == 0);
+}
+
 void fill_epi(EpiArgs& e, const sgb_conv_desc* d) {
-  e.H = d->H; e.W = d->W; e.Cout = d->Cout;
+  e.Cout = d->Cout;
   e.alpha = d->alpha; e.alpha_ptr = d->alpha_ptr; e.bias = d->bias;
   e.residual = (const bf16*)d->residual; e.res_cstride = d->res_cstride; e.res_up2 = d->res_up2; e.res_after = d->res_after_mask;
   e.res_scale = d->res_scale != 0.f ? d->res_scale : 1.f;
@@ -608,18 +581,7 @@ int pick_bn(const sgb_conv_desc* d) {
 
 // The hot epilogue shapes of the training step get compile-time variants of the kernel; every other launch takes the
 // general kernel (F = -1, run-time flags).
-template <int... Fs>
-struct FpropVariants {
-  static constexpr bool has(int f) { return ((f == Fs) || ...); }
-  static int launch(int f, int grid, size_t smem, cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                    const CUtensorMap& tmY, const CUtensorMap& tmAux, const FpropArgs& p) {
-    int rc = 0;
-    const bool hit = ((f == Fs && ((rc = launch_kernel<conv_fprop_kernel<Fs>>(grid, kThreads, smem, stream, tmA, tmB, tmY, tmAux, p)),
-                                   true)) || ...);
-    return hit ? rc : launch_kernel<conv_fprop_kernel<-1>>(grid, kThreads, smem, stream, tmA, tmB, tmY, tmAux, p);
-  }
-};
-using FpropCompiled = FpropVariants<
+using FpropCompiled = EpiVariants<
     kEpiFull,                                                          // dgrad / attention GEMMs
     kEpiFull | kEpiBias,                                               // generator convs
     kEpiFull | kEpiBias | kEpiRelu,                                    // discriminator convs (no backward expected)
@@ -693,8 +655,7 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   const int Hin = d->Hin > 0 ? d->Hin : d->H, Win = d->Win > 0 ? d->Win : d->W;
   p.out_sub = d->out_sub == 2 ? 2 : 1;
   SGB_REQUIRE(p.out_sub == 1 || (!d->residual && !d->mask));
-  p.use_tma = (p.out_sub == 1 && !d->y_fp32 && BN % 64 == 0 && d->Cout % 8 == 0 && d->y_cstride % 8 == 0 &&
-               (!d->residual || d->res_cstride % 8 == 0) && (!d->mask || d->mask_cstride % 8 == 0)) ? 1 : 0;
+  p.use_tma = (p.out_sub == 1 && epi_tma_ok(d, BN)) ? 1 : 0;
   // auxiliary epilogue operand through TMA: exactly one of residual / mask, bf16 NHWC with 16-byte aligned channel stride
   p.aux_kind = 0; p.aux_tw = p.tw; p.aux_th = p.th;
   if (p.use_tma && (d->residual != nullptr || d->mask != nullptr)) {   // (mask_bits are 8-byte direct loads)
@@ -782,7 +743,9 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
                       (pingpong ? 0 : (size_t)kTileM * acc_row_bytes(BN)) + 1024 + 8 * (2 * stages + 1 + 4 * 3);
   SGB_REQUIRE(smem <= 227u * 1024u);
   int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
-  return FpropCompiled::launch(f, grid, smem, stream, tmA, tmB, tmY, tmAux, p);
+  return FpropCompiled::launch(f, [&](auto F) {
+    return launch_kernel<conv_fprop_kernel<decltype(F)::value>>(grid, kThreads, smem, stream, tmA, tmB, tmY, tmAux, p);
+  });
 }
 
 extern "C" int sgb_conv_wgrad_fuses_dbias(const sgb_wgrad_desc* d) {

@@ -27,8 +27,6 @@ static constexpr int kRowsConsumers = 256;
 static constexpr int kRowsThreads = 128 + kRowsConsumers;  // warps 0: A producer, 2: B producer, 4..11: MMA + epilogue
 static constexpr uint32_t kRowsAccBar = 3;                 // named barrier of the consumers (1, 2: epilogue teams)
 
-__host__ __device__ inline uint32_t rows_acc_ld(int BN) { return (uint32_t)BN * 4u + 16u; }
-
 struct RowsArgs {
   int B, H, W, Cin, Cout;
   int kblocks, BN, tiles_n, segs, hpairs, num_tiles;
@@ -40,7 +38,18 @@ struct RowsArgs {
 // Shared memory in front of the operand rings: the bf16 staging tiles of the fragment epilogue, or (staged-row epilogue) the
 // fp32 accumulator rows of one output row.  A multiple of 1024 bytes.
 __host__ __device__ inline uint32_t rows_epi_bytes(const RowsArgs& p) {
-  return p.use_tma ? 2u * (uint32_t)p.epi_nbuf * 64u * 128u : 128u * rows_acc_ld(p.BN);
+  return p.use_tma ? 2u * (uint32_t)p.epi_nbuf * 64u * 128u : 128u * acc_row_bytes(p.BN);
+}
+
+// Tile index -> (channel tile, 128-pixel segment, row pair, image), channel tiles fastest.
+struct RowsTile { int nt, ws, hp, b; };
+__device__ __forceinline__ RowsTile rows_tile(const RowsArgs& p, int t) {
+  RowsTile c;
+  c.nt = t % p.tiles_n; t /= p.tiles_n;
+  c.ws = t % p.segs; t /= p.segs;
+  c.hp = t % p.hpairs; t /= p.hpairs;
+  c.b = t;
+  return c;
 }
 
 // One work item of a consumer warpgroup: both output rows' MMAs over every K block, accumulators for rows 0 / 1 in acc[0 / 1].
@@ -103,7 +112,7 @@ __device__ __forceinline__ void rows_mma_tile(const RowsArgs& p, float (&acc)[2]
 template <int BN>
 __device__ __forceinline__ void rows_stage(const float (&acc)[BN / 2], uint32_t acc_base, int wg) {
   named_bar_sync(kRowsAccBar, kRowsConsumers);
-  acc_store<BN>(acc, acc_base + (uint32_t)wg * 64u * rows_acc_ld(BN), rows_acc_ld(BN));
+  acc_store<BN>(acc, acc_base + (uint32_t)wg * 64u * acc_row_bytes(BN), acc_row_bytes(BN));
   named_bar_sync(kRowsAccBar, kRowsConsumers);
 }
 
@@ -114,7 +123,7 @@ __device__ __forceinline__ void rows_consumer(const RowsArgs& p, const CUtensorM
   const int wg = ct >> 7;
   const int q = (ct >> 5) & 3;
   const int lane = threadIdx.x & 31;
-  const float alpha = p.e.alpha_ptr ? p.e.alpha * __ldg(p.e.alpha_ptr) : p.e.alpha;
+  const float alpha = epi_alpha(p.e);
   uint32_t ita = 0, itb = 0;
   if (p.resident) mbar_wait(bar_base + 8u * (2 * p.a_stages), 0);
   if constexpr (F < 0 || BN < 64) {
@@ -123,13 +132,10 @@ __device__ __forceinline__ void rows_consumer(const RowsArgs& p, const CUtensorM
       // warpgroup 1 runs epilogue_row, one thread per pixel
       const int row = q * 32 + lane;
       const bool vec_ok = epi_vec_ok(p.e);
-      const uint32_t t_row = epi_base + (uint32_t)row * rows_acc_ld(BN);
+      const uint32_t t_row = epi_base + (uint32_t)row * acc_row_bytes(BN);
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        int t = tile;
-        const int nt = t % p.tiles_n; t /= p.tiles_n;
-        const int ws = t % p.segs; t /= p.segs;
-        const int hp = t % p.hpairs; t /= p.hpairs;
-        const int b = t;
+        const RowsTile tc = rows_tile(p, tile);
+        const int nt = tc.nt, ws = tc.ws, hp = tc.hp, b = tc.b;
         float acc[2][BN / 2];
         rows_mma_tile<BN>(p, acc, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb, ita, itb, wg);
         const int w = ws * 128 + row;
@@ -139,7 +145,7 @@ __device__ __forceinline__ void rows_consumer(const RowsArgs& p, const CUtensorM
           else rows_stage<BN>(acc[1], epi_base, wg);
           const int h = hp * 2 + j;
           const long long pix = ((long long)b * p.H + h) * p.W + w;
-          const long long rpix = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1)) : pix;
+          const long long rpix = epi_rpix(p.e, b, h, w, p.H, p.W, pix);
           if (wg == 0) epilogue_row(p.e, t_row, BN, nt * BN, true, pix, rpix, alpha, vec_ok);
         }
       }
@@ -153,11 +159,8 @@ __device__ __forceinline__ void rows_consumer(const RowsArgs& p, const CUtensorM
     const uint32_t r0 = 16u * (uint32_t)q + ((uint32_t)lane >> 2);
     uint32_t sbuf = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      int t = tile;
-      const int nt = t % p.tiles_n; t /= p.tiles_n;
-      const int ws = t % p.segs; t /= p.segs;
-      const int hp = t % p.hpairs; t /= p.hpairs;
-      const int b = t;
+      const RowsTile tc = rows_tile(p, tile);
+      const int nt = tc.nt, ws = tc.ws, hp = tc.hp, b = tc.b;
       float acc[2][BN / 2];
       rows_mma_tile<BN>(p, acc, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb, ita, itb, wg);
       const int w0 = ws * 128 + wg * 64;
@@ -169,7 +172,7 @@ __device__ __forceinline__ void rows_consumer(const RowsArgs& p, const CUtensorM
         for (int hr = 0; hr < 2; ++hr) {
           const int w = w0 + (int)r0 + 8 * hr;
           pix[hr] = ((long long)b * p.H + h) * p.W + w;
-          rpix[hr] = p.e.res_up2 ? (((long long)b * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1)) : pix[hr];
+          rpix[hr] = epi_rpix(p.e, b, h, w, p.H, p.W, pix[hr]);
         }
         epilogue_frag_tma<F, BN>(p.e, tmY, acc[j], nt * BN, w0, h, b, pix, rpix, alpha, stage, p.epi_nbuf, sbuf, 1u + wg, leader);
       }
@@ -209,14 +212,6 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   }
   __syncthreads();
 
-  auto decode = [&](int tile, int& nt, int& ws, int& hp, int& b) {
-    int t = tile;
-    nt = t % p.tiles_n; t /= p.tiles_n;
-    ws = t % p.segs; t /= p.segs;
-    hp = t % p.hpairs; t /= p.hpairs;
-    b = t;
-  };
-
   if (warp >= 4) {
     reg_alloc<kConsumerRegs>();
     switch (p.BN) {
@@ -233,9 +228,8 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       // ------------------------------------------------------------- A producer: four halo rows per K block
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        int nt, ws, hp, b;
-        decode(tile, nt, ws, hp, b);
-        const int w0 = ws * 128, h0 = hp * 2;
+        const RowsTile tc = rows_tile(p, tile);
+        const int w0 = tc.ws * 128, h0 = tc.hp * 2, b = tc.b;
         for (int kb = 0; kb < p.kblocks; ++kb, ++it) {
           const int s = it % p.a_stages;
           mbar_wait(a_empty(s), ((it / p.a_stages) & 1) ^ 1);
@@ -256,8 +250,7 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       } else {
         uint32_t it = 0;
         for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-          int nt, ws, hp, b;
-          decode(tile, nt, ws, hp, b);
+          const int nt = rows_tile(p, tile).nt;
           for (int kb = 0; kb < p.kblocks; ++kb)
             for (int tap = 0; tap < 9; ++tap, ++it) {
               const int s = it % p.b_stages;
@@ -273,6 +266,15 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 
 void fill_epi(EpiArgs& e, const sgb_conv_desc* d);
 int pick_bn(const sgb_conv_desc* d);
+bool epi_tma_ok(const sgb_conv_desc* d, int BN);
+
+using RowsCompiled = EpiVariants<
+    kEpiFull | kEpiBias,                                               // generator 3x3
+    kEpiFull | kEpiBias | kEpiRelu,                                    // discriminator 3x3
+    kEpiFull | kEpiBias | kEpiRelu | kEpiBitsOut,                      // ... writing the ReLU bit plane
+    kEpiFull | kEpiMask,                                               // dgrad through a ReLU (bf16 mask)
+    kEpiFull | kEpiMask | kEpiMaskBits,                                // dgrad through a ReLU (bit plane)
+    kEpiFull>;                                                         // plain dgrad
 
 bool conv3x3_rows_eligible(const sgb_conv_desc* d) {
   return d->KH == 3 && d->KW == 3 && d->pad_h == 1 && d->pad_w == 1 && d->w_mode == 0 && d->W % 128 == 0 && d->H % 2 == 0 &&
@@ -292,8 +294,7 @@ int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream) {
   const uint32_t budget = 227u * 1024u - 2048u;
   const uint32_t a_stage = 4 * kRowBufBytes;
   const uint32_t resident_bytes = 9u * p.kblocks * b_tile;
-  p.use_tma = (!d->y_fp32 && p.BN % 64 == 0 && d->y_cstride % 8 == 0 && (!d->residual || d->res_cstride % 8 == 0) &&
-               (!d->mask || d->mask_cstride % 8 == 0)) ? 1 : 0;
+  p.use_tma = epi_tma_ok(d, p.BN) ? 1 : 0;
   // two staging tiles per warpgroup (a chunk's store overlaps the next chunk's packing), one where that would cost the
   // resident filter its second halo stage (C = 64: 72 KiB taps + 2 x 68 KiB halo + 16 KiB staging)
   p.epi_nbuf = 2;
@@ -334,18 +335,9 @@ int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream) {
   SGB_REQUIRE(smem <= 227u * 1024u);
   const int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
   const int f = p.use_tma ? epi_flags_of(p.e) : -1;
-#define SGB_ROWS_CASE(FLAGS) \
-  case (FLAGS): return launch_kernel<conv3x3_rows_kernel<(FLAGS)>>(grid, kRowsThreads, smem, stream, tmA, tmB, tmY, p);
-  switch (f) {
-    SGB_ROWS_CASE(kEpiFull | kEpiBias)                                  // generator 3x3
-    SGB_ROWS_CASE(kEpiFull | kEpiBias | kEpiRelu)                       // discriminator 3x3
-    SGB_ROWS_CASE(kEpiFull | kEpiBias | kEpiRelu | kEpiBitsOut)         // ... writing the ReLU bit plane
-    SGB_ROWS_CASE(kEpiFull | kEpiMask)                                  // dgrad through a ReLU (bf16 mask)
-    SGB_ROWS_CASE(kEpiFull | kEpiMask | kEpiMaskBits)                   // dgrad through a ReLU (bit plane)
-    SGB_ROWS_CASE(kEpiFull)                                             // plain dgrad
-    default: return launch_kernel<conv3x3_rows_kernel<-1>>(grid, kRowsThreads, smem, stream, tmA, tmB, tmY, p);
-  }
-#undef SGB_ROWS_CASE
+  return RowsCompiled::launch(f, [&](auto F) {
+    return launch_kernel<conv3x3_rows_kernel<decltype(F)::value>>(grid, kRowsThreads, smem, stream, tmA, tmB, tmY, p);
+  });
 }
 
 }  // namespace sgb

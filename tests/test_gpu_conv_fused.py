@@ -69,7 +69,7 @@ def _flags(s):
     return -1 if s == "general" else sum(FLAG[t] for t in s.split("|"))
 
 
-# The compiled variants (FpropCompiled in csrc/umma_conv.cu, the SGB_ROWS_CASE switch in csrc/umma_conv3x3.cu).
+# The compiled variants (FpropCompiled in csrc/umma_conv.cu, RowsCompiled in csrc/umma_conv3x3.cu).
 FPROP_VARIANTS = {_flags(s) for s in (
     "Full", "Full|Bias", "Full|Bias|Relu", "Full|Bias|Relu|BitsOut", "Full|ResPre|AuxRes", "Full|Bias|ResPre|AuxRes",
     "Full|Bias|Relu|ResPre|AuxRes", "Full|Bias|Relu|ResPre|AuxRes|BitsOut", "Full|Mask|MaskBits",
