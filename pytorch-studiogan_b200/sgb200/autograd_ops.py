@@ -48,13 +48,31 @@ class TFunction(Function):
 def _direct_grad(p):
     """The arena-backed ``.grad`` of a leaf parameter that opted in (utils/arena.GradArena.attach), else None.  ConvFn then
     adds its weight gradient there itself and reports no gradient to autograd, which would otherwise launch one tiny add
-    per parameter and backward pass (~1.6 k per step for BigGAN-Deep)."""
-    if not getattr(p, "_sgb_direct_grad", False) or not p.is_leaf or torch.is_grad_enabled():
+    per parameter and backward pass (~1.6 k per step for BigGAN-Deep).  Frozen parameters keep their arena slot, so the
+    batched spectral-norm backward may address it (their pass buffer holds zeros)."""
+    if not getattr(p, "_sgb_direct_grad", False) or not p.is_leaf:
         return None
     g = p.grad
     if g is None or g.dtype != torch.float32 or not g.is_contiguous() or g.shape != p.shape:
         return None
     return g
+
+
+def _sn_packs(weight, cfg, Cout, Cin, taps, need_dx, need_dw, perm_S=1):
+    """(fprop pack, dgrad pack, sigma, u, v) of a conv weight, u / v as the chain rule of this forward needs them.  The
+    network's batched spectral-norm pass leaves them in cfg['sn_cache'] (its dgrad pack is None only when gradients are
+    off, and then no op needs it); stand-alone use runs the per-layer kernels."""
+    cache = cfg.get("sn_cache")
+    if cache is not None:
+        return cache
+    sn = cfg.get("sn")
+    sigma = us = vs = None
+    if sn is not None:
+        sigma = sn.sigma(cfg.get("do_power_iteration", True))
+        if need_dw:
+            us, vs = sn.module.weight_u.clone(), sn.module.weight_v.clone()
+    wf, wd = K.weight_pack(weight, sigma, Cout, Cin, taps, True, need_dx, perm_S)
+    return wf, wd, sigma, us, vs
 
 
 def _tadd(a, b):
@@ -73,13 +91,16 @@ class SpectralNormState:
         self.eps = eps
         self.ws = None
 
-    def tensors(self):
+    def sigma(self, do_power_iteration):
+        """One power iteration of the module's u / v (do_power_iteration) and sigma = u . (W v), a [1] fp32 tensor."""
         m = self.module
         W = m.weight_orig
         if self.ws is None or self.ws.device != W.device:
             R = W.shape[0]
             self.ws = K.sn_workspace(R, W.numel() // R, W.device)
-        return m.weight_u, m.weight_v, self.ws
+        sigma = torch.empty(1, device=W.device, dtype=torch.float32)
+        K.sn_power_iter(W.detach(), m.weight_u, m.weight_v, sigma, self.ws, self.eps, do_power_iteration)
+        return sigma
 
 
 def _grad_bf16(dy):
@@ -95,17 +116,6 @@ def _grad_bf16(dy):
     return K.as_nhwc(dy)
 
 
-def _direct_grad_ptr(p):
-    """Device address of the arena-backed ``.grad`` of a parameter (see _direct_grad), else None.  Frozen parameters keep
-    their arena slot, so the batched spectral-norm backward may address it (their pass buffer holds zeros)."""
-    if not getattr(p, "_sgb_direct_grad", False) or not p.is_leaf:
-        return None
-    g = p.grad
-    if g is None or g.dtype != torch.float32 or not g.is_contiguous() or g.shape != p.shape:
-        return None
-    return g.data_ptr()
-
-
 def conv_param_grads(x, dz, weight, need_w, need_b, KH, KW, pad, dims, sigma, u_saved, v_saved, perm_S=1, sn_pass=None, bias=None):
     """Weight and bias gradient of y = conv(x, W / sigma) + b given dz = dL/dy (NHWC bf16): wgmma weight-gradient kernel,
     then the spectral-norm chain rule (sgb_sn_backward).  The weight gradient is added straight into the flat gradient
@@ -114,7 +124,9 @@ def conv_param_grads(x, dz, weight, need_w, need_b, KH, KW, pad, dims, sigma, u_
     back to a reduction pass."""
     Cout, Cin, taps = dims
     dW = dbias = None
-    if need_w and sn_pass is not None and sn_pass[0] is not None and _direct_grad(weight) is not None and sn_pass[0].usable():
+    # while autograd records (double backward) the gradient must reach it as a tensor, not be added into the arena
+    tgt = _direct_grad(weight) if (need_w and not torch.is_grad_enabled()) else None
+    if tgt is not None and sn_pass is not None and sn_pass[0] is not None and sn_pass[0].usable():
         # batched path: accumulate the raw weight gradient into this forward pass's flat buffer; the spectral-norm chain
         # rule of ALL layers runs as one launch pair when the backward pass ends (snbatch._Pass.flush)
         G = sn_pass[0].g_slice(sn_pass[1])
@@ -137,7 +149,6 @@ def conv_param_grads(x, dz, weight, need_w, need_b, KH, KW, pad, dims, sigma, u_
                 dbias = dbias[:Cout]
         else:
             G = K.conv_wgrad(x, dz, KH, KW, pad, pad)
-        tgt = _direct_grad(weight)
         if tgt is not None:       # accumulate straight into the flat gradient arena: no per-parameter add kernel
             K.sn_backward(G, weight, u_saved, v_saved, sigma, Cout, Cin, taps, perm_S, out=tgt)
         else:
@@ -160,20 +171,9 @@ class ConvFn(TFunction):
         Cout = weight.shape[0]
         Cin = weight.numel() // (Cout * KH * KW)
         taps = KH * KW
-        sn = cfg.get("sn")
-        sigma = u_saved = v_saved = None
         need_dx = ctx.needs_input_grad[0]
-        need_dw = ctx.needs_input_grad[1]
-        cache = cfg.get("sn_cache")
-        if cache is not None:                       # power iteration + packs already done by the network's batched pass
-            wf, wd, sigma, u_saved, v_saved = cache
-            u = v = None
-        else:
-            if sn is not None:
-                u, v, ws = sn.tensors()
-                sigma = torch.empty(1, device=weight.device, dtype=torch.float32)
-                K.sn_power_iter(weight, u, v, sigma, ws, sn.eps, cfg.get("do_power_iteration", True))
-            wf, wd = K.weight_pack(weight, sigma, Cout, Cin, taps, True, need_dx, cfg.get("perm_S", 1))
+        wf, wd, sigma, u_saved, v_saved = _sn_packs(weight, cfg, Cout, Cin, taps, need_dx, ctx.needs_input_grad[1],
+                                                    cfg.get("perm_S", 1))
         Cout_p = K.pad8(Cout)
         res = residual
         y = K.conv_fprop(x, wf, Cout_p, KH, KW, pad, pad, bias=bias if Cout_p == Cout else _pad_bias(bias, Cout_p),
@@ -181,8 +181,6 @@ class ConvFn(TFunction):
                          out_fp32=cfg.get("out_fp32", False), stride=cfg.get("stride", 1),
                          want_relu_bits=cfg.get("premasked", False) and any(ctx.needs_input_grad))
         ctx.x_bits = getattr(x, "_sgb_relu_bits", None) if (need_dx and cfg.get("mask_input", False)) else None
-        if need_dw and sn is not None and cache is None:
-            u_saved, v_saved = u.clone(), v.clone()
         ctx.cfg = cfg
         ctx.dims = (Cout, Cin, taps)
         ctx.bias_ref = bias                          # the parameter object (arena-backed .grad), not a saved activation
@@ -562,23 +560,6 @@ class ReluPassFn(TFunction):
         return da0
 
 
-def _sn_packs(weight, cfg, Cout, Cin, taps, need_dx):
-    """(fprop pack, dgrad pack, sigma, u, v) of a conv weight: the network's batched spectral-norm pass left them in
-    cfg['sn_cache']; stand-alone use runs the per-layer kernels."""
-    cache = cfg.get("sn_cache")
-    if cache is not None:
-        return cache
-    sn = cfg.get("sn")
-    sigma = us = vs = None
-    if sn is not None:
-        u, v, ws = sn.tensors()
-        sigma = torch.empty(1, device=weight.device, dtype=torch.float32)
-        K.sn_power_iter(weight, u, v, sigma, ws, sn.eps, cfg.get("do_power_iteration", True))
-        us, vs = u.clone(), v.clone()
-    wf, wd = K.weight_pack(weight, sigma, Cout, Cin, taps, True, need_dx)
-    return wf, wd, sigma, us, vs
-
-
 class DEntryConvFn(TFunction):
     """Entry of a BigGAN-Deep discriminator block (src/models/big_resnet_deep_legacy.py:211-224) as one op:
          a0 (= relu(block input); the producer's epilogue applied the in-place ReLU) ->
@@ -592,7 +573,7 @@ class DEntryConvFn(TFunction):
     def forward(ctx, a0, weight, bias, cfg):
         B, Cin, H, W, _ = K.geom(a0)
         hid = weight.shape[0]
-        wf, wd, sigma, us, vs = _sn_packs(weight, cfg, hid, Cin, 1, True)
+        wf, wd, sigma, us, vs = _sn_packs(weight, cfg, hid, Cin, 1, True, ctx.needs_input_grad[1])
         h1 = K.conv_fprop(a0, wf, hid, 1, 1, 0, 0, bias=bias, relu=True, want_relu_bits=any(ctx.needs_input_grad))
         ctx.a0_bits = getattr(a0, "_sgb_relu_bits", None) if ctx.needs_input_grad[0] else None
         down = cfg["downsample"]
@@ -636,25 +617,12 @@ class ConcatSkipFn(TFunction):
     def forward(ctx, px, weight, bias, cfg):
         B, Cin, H, W, _ = K.geom(px)
         Cextra = weight.shape[0]
-        sn = cfg.get("sn")
-        sigma = u_saved = v_saved = None
-        need_dx = ctx.needs_input_grad[0]
-        cache = cfg.get("sn_cache")
-        if cache is not None:
-            wf, wd, sigma, u_saved, v_saved = cache
-        else:
-            if sn is not None:
-                u, v, ws = sn.tensors()
-                sigma = torch.empty(1, device=weight.device, dtype=torch.float32)
-                K.sn_power_iter(weight, u, v, sigma, ws, sn.eps, cfg.get("do_power_iteration", True))
-            wf, wd = K.weight_pack(weight, sigma, Cextra, Cin, 1, True, need_dx)
+        wf, wd, sigma, u_saved, v_saved = _sn_packs(weight, cfg, Cextra, Cin, 1, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
         skip = getattr(px, "_sgb_concat_buf", None)       # DEntryConvFn pooled straight into the concat buffer
         if skip is None or skip.shape[1] != Cin + Cextra:
             skip = K.empty_nhwc(B, Cin + Cextra, H, W, px.device)
             K.axpby(px, out=skip[:, :Cin])
         K.conv_fprop(skip[:, :Cin], wf, Cextra, 1, 1, 0, 0, bias=bias, out=skip[:, Cin:])
-        if ctx.needs_input_grad[1] and sn is not None and cache is None:
-            u_saved, v_saved = u.clone(), v.clone()
         ctx.cfg = cfg
         ctx.dims = (Cextra, Cin)
         ctx.bias_ref = bias
@@ -722,15 +690,12 @@ class DHeadFn(TFunction):
         if reuse is not None:
             s1, u1, v1, sE, uE, vE = reuse
         else:
-            def power(w, sn):
+            def power(sn):
                 if sn is None:
                     return None, None, None
-                u, v, ws = sn.tensors()
-                sg = torch.empty(1, device=w.device, dtype=torch.float32)
-                K.sn_power_iter(w.detach(), u, v, sg, ws, sn.eps, cfg.get("training", True))
-                return sg, u.clone(), v.clone()
-            s1, u1, v1 = power(w1, cfg.get("sn1"))
-            sE, uE, vE = power(E, cfg.get("snE")) if E is not None else (None, None, None)
+                return sn.sigma(cfg.get("training", True)), sn.module.weight_u.clone(), sn.module.weight_v.clone()
+            s1, u1, v1 = power(cfg.get("sn1"))
+            sE, uE, vE = power(cfg.get("snE")) if E is not None else (None, None, None)
         cfg["saved"] = (s1, u1, v1, sE, uE, vE)
         adv = K.dhead_fwd(h, w1, s1, None if cfg.get("no_bias", False) else b1, E, sE, labels)
         ctx.has_E = E is not None
@@ -851,20 +816,8 @@ class SelfAttentionFn(TFunction):
         N, M = H * W, (H // 2) * (W // 2)
         packs = []
         sn_saved = []
-        for w, cfg, cin, cout in ((w_theta, cfgs[0], C, c8), (w_phi, cfgs[1], C, c8), (w_g, cfgs[2], C, c2), (w_o, cfgs[3], c2, C)):
-            sn = cfg.get("sn")
-            sg = None
-            us = vs = None
-            cache = cfg.get("sn_cache")
-            if cache is not None and cache[1] is not None:
-                wf, wd, sg, us, vs = cache
-            else:
-                if sn is not None:
-                    u, v, ws = sn.tensors()
-                    sg = torch.empty(1, device=w.device, dtype=torch.float32)
-                    K.sn_power_iter(w, u, v, sg, ws, sn.eps, cfg.get("do_power_iteration", True))
-                    us, vs = u.clone(), v.clone()
-                wf, wd = K.weight_pack(w, sg, cout, cin, 1, True, True)
+        for i, (w, cin, cout) in enumerate(((w_theta, C, c8), (w_phi, C, c8), (w_g, C, c2), (w_o, c2, C))):
+            wf, wd, sg, us, vs = _sn_packs(w, cfgs[i], cout, cin, 1, True, ctx.needs_input_grad[1 + i])
             packs.append((wf, wd))
             sn_saved.append((sg, us, vs))
         theta = K.conv_fprop(x, packs[0][0], c8, 1, 1, 0, 0)                      # [B, c8, H, W]
@@ -884,6 +837,7 @@ class SelfAttentionFn(TFunction):
         t = K.conv_fprop(o, packs[3][0], C, 1, 1, 0, 0)                           # conv1x1_attn
         out = K.axpby(t, x, a=1.0, a_dev=sigma, b=1.0)
         ctx.dims = (B, C, H, W, c8, c2, N, M)
+        ctx.cfgs = cfgs
         ctx.sn_saved = sn_saved
         ctx.packs = packs
         ctx.save_for_backward(x, theta, phi_f, phi, g_f, g, S, o, t, sigma, w_theta, w_phi, w_g, w_o)
@@ -899,7 +853,6 @@ class SelfAttentionFn(TFunction):
         dt = K.axpby(dout, a=1.0, a_dev=sigma)
         # conv1x1_attn
         do = K.conv_fprop(dt, packs[3][1], c2, 1, 1, 0, 0)
-        G_o = K.conv_wgrad(o, dt, 1, 1, 0, 0)
         # o = P . g   ->  dP = do . g^T (keys as output channels), dg = P^T . do (per image)
         dg_pool = K.conv_wgrad(do, P, 1, 1, 0, 0, per_image=True)                 # [B][M][1][c2] fp32
         if M % 64 == 0:
@@ -919,15 +872,13 @@ class SelfAttentionFn(TFunction):
         dx = K.conv_fprop(dtheta, packs[0][1], C, 1, 1, 0, 0, residual=dout)
         dx = K.conv_fprop(dphi_f, packs[1][1], C, 1, 1, 0, 0, residual=dx)
         dx = K.conv_fprop(dg_f, packs[2][1], C, 1, 1, 0, 0, residual=dx)
-        grads_w = []
-        for (w, xin, dyv, cout, cin, idx) in ((w_theta, x, dtheta, c8, C, 0), (w_phi, x, dphi_f, c8, C, 1), (w_g, x, dg_f, c2, C, 2),
-                                              (w_o, o, None, C, c2, 3)):
-            if not ctx.needs_input_grad[1 + idx]:
-                grads_w.append(None)
-                continue
-            G = G_o if idx == 3 else K.conv_wgrad(xin, dyv, 1, 1, 0, 0)
-            sg, us, vs = sn_saved[idx]
-            grads_w.append(K.sn_backward(G, w, us, vs, sg, cout, cin, 1))
+        grads_w = [None] * 4
+        if not SKIP_PARAM_GRADS:
+            for i, (w, xin, dz, cout, cin) in enumerate(((w_theta, x, dtheta, c8, C), (w_phi, x, dphi_f, c8, C), (w_g, x, dg_f, c2, C),
+                                                         (w_o, o, dt, C, c2))):
+                sg, us, vs = sn_saved[i]
+                grads_w[i], _ = conv_param_grads(xin, dz, w, ctx.needs_input_grad[1 + i], False, 1, 1, 0, (cout, cin, 1), sg, us, vs,
+                                                 1, ctx.cfgs[i].get("sn_pass"))
         return dx, grads_w[0], grads_w[1], grads_w[2], grads_w[3], dsigma, None
 
 

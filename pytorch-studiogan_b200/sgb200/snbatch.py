@@ -162,10 +162,11 @@ class SNBatch:
     def bwd_table(self):
         """Device table for sgb_sn_backward_batch, valid while every layer's ``.grad`` is its view of the flat gradient arena
         (utils/arena.GradArena.attach); None otherwise (the per-layer path is used then)."""
-        from .autograd_ops import _direct_grad_ptr
-        key = tuple(_direct_grad_ptr(w) for w in self.params)
-        if any(k is None for k in key):
+        from .autograd_ops import _direct_grad
+        grads = [_direct_grad(w) for w in self.params]
+        if any(g is None for g in grads):
             return None
+        key = tuple(g.data_ptr() for g in grads)
         if key != self._bwd_key:
             bt = self._bwd_host.copy()
             for i, k in enumerate(key):

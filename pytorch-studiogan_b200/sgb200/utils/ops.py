@@ -11,7 +11,6 @@ import torch.nn.functional as F
 from torch.nn import init
 
 from .. import autograd_ops as A
-from .. import kernels as K
 
 SN_EPS = 1e-6  # src/utils/ops.py:204,216,220,224
 
@@ -33,6 +32,17 @@ def _apply_spectral_norm(module, eps=SN_EPS):
 
 def _w(module):
     return module.weight_orig if hasattr(module, "weight_orig") else module.weight
+
+
+def _sn_divided(module):
+    """W / sigma of a spectrally-normalised module whose weight is used as a tensor (image convs, embeddings, head layers):
+    sigma from the library's power iteration (in train mode, as the reference's hook); where W needs a gradient, sigma is
+    formed again as u . (W v) with u, v held constant, so that the gradient reaches ``weight_orig`` through ordinary autograd."""
+    W = module.weight_orig
+    sigma = module._sn.sigma(module.training)
+    if torch.is_grad_enabled() and W.requires_grad:
+        sigma = torch.dot(module.weight_u.detach().clone(), torch.mv(W.reshape(W.shape[0], -1), module.weight_v.detach().clone()))
+    return W / sigma
 
 
 class _ConvBase(nn.Conv2d):
@@ -61,17 +71,8 @@ class _ConvBase(nn.Conv2d):
     def _forward_image(self, x_col, residual, relu, premasked):
         """3 -> C convolution on an image: ``x_col`` is the [B, 32, H, W] patch tensor from ImageColFn and the layer runs
         as a K = 32 GEMM.  The [Cout, 3, 3, 3] weight (864..3456 numbers) is re-ordered to [Cout, (tap, c)] with tensor
-        ops; its spectral norm uses the library's power iteration and the reference's sigma = u . (W v) with u, v held
-        constant, so the gradient reaches ``weight_orig`` through ordinary autograd."""
-        W = _w(self)
-        sn = getattr(self, "_sn", None)
-        if sn is not None:
-            u, v, ws = sn.tensors()
-            sigma = torch.empty(1, device=W.device, dtype=torch.float32)
-            K.sn_power_iter(W.detach(), u, v, sigma, ws, sn.eps, self.training)
-            if torch.is_grad_enabled() and W.requires_grad:
-                sigma = torch.dot(u.detach().clone(), torch.mv(W.reshape(W.shape[0], -1), v.detach().clone()))
-            W = W / sigma
+        ops (spectral norm: _sn_divided)."""
+        W = _sn_divided(self) if hasattr(self, "_sn") else self.weight
         Wp = W.permute(0, 2, 3, 1).reshape(W.shape[0], 27)
         cfg = {"KH": 1, "KW": 1, "pad": 0, "relu": relu, "premasked": premasked, "sn": None}
         return A.ConvFn.call(x_col, Wp, self.bias, residual, cfg)
@@ -128,15 +129,7 @@ class SNEmbedding(nn.Embedding):
         _apply_spectral_norm(self)
 
     def forward(self, label):
-        W = self.weight_orig
-        u, v, ws = self._sn.tensors()
-        sigma = torch.empty(1, device=W.device, dtype=torch.float32)
-        K.sn_power_iter(W.detach(), u, v, sigma, ws, self._sn.eps, self.training)
-        if not torch.is_grad_enabled() or not W.requires_grad:
-            return F.embedding(label, W.detach()) / sigma
-        # sigma = u^T W v with u, v constant: keep the dependence of sigma on W for the gradient
-        sig = torch.dot(u.detach().clone(), torch.mv(W, v.detach().clone()))
-        return F.embedding(label, W) / sig
+        return F.embedding(label, _sn_divided(self))
 
 
 def conv2d(in_channels, out_channels, kernel_size, stride=1, padding=0, dilation=1, groups=1, bias=True):
@@ -324,16 +317,7 @@ _HEAD_KEYS = ["embed", "proxy", "cls_output", "mi_embed", "mi_proxy", "mi_cls_ou
 
 
 def _head_weight(module):
-    W = _w(module)
-    sn = getattr(module, "_sn", None)
-    if sn is None:
-        return W
-    u, v, ws = sn.tensors()
-    sigma = torch.empty(1, device=W.device, dtype=torch.float32)
-    K.sn_power_iter(W.detach(), u, v, sigma, ws, sn.eps, module.training)
-    if torch.is_grad_enabled() and W.requires_grad:
-        sigma = torch.dot(u.detach().clone(), torch.mv(W.reshape(W.shape[0], -1), v.detach().clone()))
-    return W / sigma
+    return _sn_divided(module) if hasattr(module, "_sn") else module.weight
 
 
 class _HeadTangent:

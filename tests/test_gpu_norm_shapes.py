@@ -328,10 +328,9 @@ def _pack_rows(Cout, S, dev):
     return (co % S) * (Cout // S) + co // S if S > 1 else co
 
 
-def _check_packs(m, W3, S, sigma):
-    """Both packs of this forward must be bf16(W * (1 / sigma)) bit for bit ((1 / sigma) in fp32), zero-padded."""
+def _check_packs(wf, wd, W3, S, sigma):
+    """Both packs must be bf16(W * (1 / sigma)) bit for bit ((1 / sigma) in fp32), zero-padded."""
     from sgb200 import kernels as K
-    wf, wd = m._sn_cache[0], m._sn_cache[1]
     Cout, Cin, taps = W3.shape
     inv = (torch.ones(1) / sigma.detach().float().cpu()).to(W3.device) if sigma is not None else torch.ones(1, device=W3.device)
     Wb = (W3 * inv).to(bf16)
@@ -361,7 +360,7 @@ def _sn_forward_checks(net, label):
         if st is not None:     # u . s with u, s far from aligned cancels: the bound is relative to |u| |s| = |s|
             s = W3.reshape(Cout, -1).double() @ st[1].double()
             worst["sigma_eval"] = max(worst["sigma_eval"], abs(float(sig) - float(st[0].double() @ s)) / float(s.norm()))
-        _check_packs(m, W3, S, sig)
+        _check_packs(m._sn_cache[0], m._sn_cache[1], W3, S, sig)
     net.train()
     for call in range(2):
         with torch.enable_grad():
@@ -369,7 +368,7 @@ def _sn_forward_checks(net, label):
         for m, st in zip(mods, state):
             W3, Cout, Cin, taps, S = _geom(m)
             sig = m._sn_cache[2]
-            _check_packs(m, W3, S, sig)
+            _check_packs(m._sn_cache[0], m._sn_cache[1], W3, S, sig)
             if st is None:
                 assert sig is None
                 continue
@@ -445,6 +444,55 @@ def _sn_backward_checks(net, label, per_layer):
     assert worst <= 1e-5 and worst_single <= 1e-5
 
 
+def _one_iteration(W3, u0):
+    """float64 power iteration from u0: (u, v, sigma)."""
+    from sgb200.utils import ops
+    Wm = W3.reshape(W3.shape[0], -1).double()
+    v = F.normalize(Wm.t() @ u0.double(), dim=0, eps=ops.SN_EPS)
+    s = Wm @ v
+    u = F.normalize(s, dim=0, eps=ops.SN_EPS)
+    return u, v, float(u @ s)
+
+
+def _sn_per_layer_checks(net, label):
+    """The per-layer entry points on every layer: K.sn_power_iter from a fresh workspace, called twice (its tickets and
+    accumulator must reset), each call against float64 from the state before it; then both K.weight_pack packs."""
+    from sgb200 import kernels as K
+    from sgb200.utils import ops
+    worst = {"u": 0.0, "v": 0.0, "sigma": 0.0}
+    for m in net._snb.mods:
+        W3, Cout, Cin, taps, S = _geom(m)
+        W = ops._w(m).detach()
+        sigma = None
+        if hasattr(m, "_sn"):
+            u, v = m.weight_u.clone(), m.weight_v.clone()
+            ws = K.sn_workspace(Cout, Cin * taps, W.device)
+            sigma = torch.empty(1, device=W.device)
+            for call in range(2):
+                u_ref, v_ref, s_ref = _one_iteration(W3, u)
+                K.sn_power_iter(W, u, v, sigma, ws, ops.SN_EPS, True)
+                worst["u"] = max(worst["u"], rel_err(u, u_ref))
+                worst["v"] = max(worst["v"], rel_err(v, v_ref))
+                worst["sigma"] = max(worst["sigma"], abs(float(sigma) - s_ref) / s_ref)
+        wf, wd = K.weight_pack(W, sigma, Cout, Cin, taps, True, True, S)
+        _check_packs(wf, wd, W3, S, sigma)
+    print("%s per-layer power iteration: %s" % (label, worst))
+    assert worst["u"] <= 1e-4 and worst["v"] <= 1e-4 and worst["sigma"] <= 1e-5
+
+
+def _flagship_nets(dev):
+    """Generator and discriminator of configs/BigGAN-Deep-256res.yaml (without the EMA copy), and the configuration."""
+    from sgb200 import config as C
+    from sgb200.models import model as M
+    cfgs = C.Configurations(os.path.join(PKG, "configs", "BigGAN-Deep-256res.yaml"))
+    MODEL = copy.copy(cfgs.MODEL)
+    MODEL.apply_g_ema = False
+    torch.manual_seed(0)
+    G, _, _, D, _, _, _, _ = M.load_generator_discriminator(cfgs.DATA, cfgs.OPTIMIZATION, MODEL, cfgs.STYLEGAN, cfgs.MODULES,
+                                                           cfgs.RUN, dev, None)
+    return G, D, cfgs
+
+
 def _attach_arena(net):
     from sgb200.utils.optim import ArenaAdam
     opt = ArenaAdam(net, lr=2e-4, betas=(0.0, 0.999), eps=1e-6)
@@ -457,15 +505,8 @@ def test_spectral_norm_every_flagship_layer_vs_float64():
     generator and 56 discriminator layers of the batched spectral norm -- u, v, sigma, both weight packs (including the
     perm_S = 16 row order of linear0), a second call (tickets and workspace reset), an eval call, and the batched
     chain rule."""
-    from sgb200 import config as C
-    from sgb200.models import model as M
     dev = _cuda()
-    cfgs = C.Configurations(os.path.join(PKG, "configs", "BigGAN-Deep-256res.yaml"))
-    MODEL = copy.copy(cfgs.MODEL)
-    MODEL.apply_g_ema = False
-    torch.manual_seed(0)
-    G, _, _, D, _, _, _, _ = M.load_generator_discriminator(cfgs.DATA, cfgs.OPTIMIZATION, MODEL, cfgs.STYLEGAN, cfgs.MODULES,
-                                                           cfgs.RUN, dev, None)
+    G, D, _ = _flagship_nets(dev)
     for net, label, n in ((G, "G", 150), (D, "D", 56)):
         _attach_arena(net)
         _sn_forward_checks(net, label)
@@ -476,6 +517,38 @@ def test_spectral_norm_every_flagship_layer_vs_float64():
         pick = sorted(set([0, len(mods) // 2, len(mods) - 1] + perm + [i for i, m in enumerate(mods) if _geom(m)[3] == 9][:1]))
         _sn_backward_checks(net, label, pick)
         net._snb.clear()
+
+
+def test_no_grad_attention_generator_iterates_each_layer_once():
+    """A gradient-free forward of the flagship generator in evaluation mode as misc.make_GAN_untrainable sets it (eval(),
+    then the convs / linears back in train mode so that the power iteration runs, as in the reference): FID / IS / PRDC
+    sampling and standing statistics.  The attention convs must take one power iteration per forward like every other
+    layer.  Their weights are re-drawn from N(0, 1): for the orthogonal initialisation u is a fixed point of the iteration,
+    and a second iteration would not show."""
+    from sgb200.utils import misc, ops
+    dev = _cuda()
+    G, _, cfgs = _flagship_nets(dev)
+    G.eval()
+    G.apply(misc.set_deterministic_op_trainable)
+    attn = [c for sa in G.modules() if isinstance(sa, ops.SelfAttention)
+            for c in (sa.conv1x1_theta, sa.conv1x1_phi, sa.conv1x1_g, sa.conv1x1_attn)]
+    assert attn and all(hasattr(c, "_sn") for c in attn)
+    gen = torch.Generator(device=dev).manual_seed(15)
+    with torch.no_grad():
+        for c in attn:
+            ops._w(c).copy_(torch.randn(ops._w(c).shape, generator=gen, device=dev))
+    before = [(_geom(c)[0], c.weight_u.clone()) for c in attn]
+    z = torch.randn((2, cfgs.MODEL.z_dim), generator=gen, device=dev)
+    y = torch.randint(0, cfgs.DATA.num_classes, (2,), generator=gen, device=dev)
+    with torch.no_grad():
+        G(z, y, eval=True)
+    worst = {"u": 0.0, "v": 0.0}
+    for c, (W3, u0) in zip(attn, before):
+        u_ref, v_ref, _ = _one_iteration(W3, u0)
+        worst["u"] = max(worst["u"], rel_err(c.weight_u, u_ref))
+        worst["v"] = max(worst["v"], rel_err(c.weight_v, v_ref))
+    print("no-grad attention generator (%d convs): %s" % (len(attn), worst))
+    assert worst["u"] <= 1e-4 and worst["v"] <= 1e-4
 
 
 class _EdgeLayers(nn.Module):
@@ -496,12 +569,13 @@ class _EdgeLayers(nn.Module):
 
 def test_spectral_norm_edge_layers_vs_float64():
     """Layers the flagship does not have: pseudo tiles, odd channel counts, the unstaged backward, a layer without
-    spectral norm and a layer with more Wt.u tiles than blocks in the batched power iteration."""
+    spectral norm and a layer with more Wt.u tiles than blocks in the batched power iteration; batched and per-layer."""
     dev = _cuda()
     torch.manual_seed(5)
     net = _EdgeLayers().to(dev)
     _attach_arena(net)
     _sn_forward_checks(net, "edge")
+    _sn_per_layer_checks(net, "edge")
     _sn_backward_checks(net, "edge", list(range(len(net._snb.mods))))
     net._snb.clear()
 
