@@ -17,12 +17,6 @@
 
 namespace sgb {
 
-static inline int aug_blocks(long long work) {
-  long long b = (work + 255) / 256;
-  const long long cap = 16LL * sm_count();
-  return (int)(b < 1 ? 1 : (b > cap ? cap : b));
-}
-
 // mean over (c, h, w) of each sample: one block per (sample, slice), atomics into out[b] (pre-zeroed); scaled by 1 / n_per.
 __global__ void __launch_bounds__(256) sample_mean_kernel(const float* __restrict__ x, long long n_per, float* __restrict__ out,
                                                            int slices) {
@@ -31,7 +25,7 @@ __global__ void __launch_bounds__(256) sample_mean_kernel(const float* __restric
   const float* xp = x + (long long)b * n_per;
   float acc = 0.f;
   for (long long i = (long long)sl * 256 + threadIdx.x; i < n_per; i += (long long)slices * 256) acc += __ldg(xp + i);
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xFFFFFFFFu, acc, o);
+  acc = warp_sum(acc);
   if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = acc;
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -164,7 +158,7 @@ extern "C" int sgb_diffaug_fwd(const float* x, const float* params, const float*
   cudaStream_t stream = (cudaStream_t)stream_;
   SGB_REQUIRE(x && params && y && B > 0 && H > 0 && W > 0 && (!do_color || mean_x));
   AugGeom g = {B, 3, H, W, (int)(H * 0.5 + 0.5), (int)(W * 0.5 + 0.5)};
-  diffaug_fwd_kernel<<<aug_blocks((long long)B * H * W), 256, 0, stream>>>(x, params, mean_x, y, g, do_color, do_translation, do_cutout);
+  diffaug_fwd_kernel<<<ew_blocks((long long)B * H * W), 256, 0, stream>>>(x, params, mean_x, y, g, do_color, do_translation, do_cutout);
   SGB_LAUNCH_CHECK();
   return SGB_OK;
 }
@@ -174,12 +168,12 @@ extern "C" int sgb_diffaug_bwd(const float* dy, const float* params, float* dx, 
   cudaStream_t stream = (cudaStream_t)stream_;
   SGB_REQUIRE(dy && params && dx && B > 0 && H > 0 && W > 0 && (!do_color || mean_ws));
   AugGeom g = {B, 3, H, W, (int)(H * 0.5 + 0.5), (int)(W * 0.5 + 0.5)};
-  diffaug_bwd_gather_kernel<<<aug_blocks((long long)B * H * W), 256, 0, stream>>>(dy, params, dx, g, do_translation, do_cutout);
+  diffaug_bwd_gather_kernel<<<ew_blocks((long long)B * H * W), 256, 0, stream>>>(dy, params, dx, g, do_translation, do_cutout);
   SGB_LAUNCH_CHECK();
   if (do_color) {
     int rc = sgb_sample_mean(dx, B, (int64_t)3 * H * W, mean_ws, stream_);
     if (rc) return rc;
-    diffaug_bwd_color_kernel<<<aug_blocks((long long)B * H * W), 256, 0, stream>>>(dx, params, mean_ws, g);
+    diffaug_bwd_color_kernel<<<ew_blocks((long long)B * H * W), 256, 0, stream>>>(dx, params, mean_ws, g);
     SGB_LAUNCH_CHECK();
   }
   return SGB_OK;
@@ -189,7 +183,7 @@ extern "C" int sgb_cr_aug(const float* x, const uint8_t* flip, const int32_t* tx
                           int32_t H, int32_t W, sgb_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   SGB_REQUIRE(x && y && B > 0 && C > 0 && H > 1 && W > 1);
-  cr_aug_kernel<<<aug_blocks((long long)B * C * H * W), 256, 0, stream>>>(x, flip, tx, ty, y, B, C, H, W);
+  cr_aug_kernel<<<ew_blocks((long long)B * C * H * W), 256, 0, stream>>>(x, flip, tx, ty, y, B, C, H, W);
   SGB_LAUNCH_CHECK();
   return SGB_OK;
 }

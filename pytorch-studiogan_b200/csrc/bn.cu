@@ -7,26 +7,29 @@
 // Reference arithmetic: src/utils/ops.py:14-28 (ConditionalBatchNorm2d), :227-228 (batchnorm_2d, eps 1e-4,
 // momentum 0.1), torch F.batch_norm; cross-rank reduction points follow torch/nn/modules/_functions.py:7-212.
 #include "common.cuh"
+#include <type_traits>
 
 namespace sgb {
 
-__device__ __forceinline__ void unpack8(const uint4& r, float (&f)[8]) {
-  f[0] = __uint_as_float(r.x << 16); f[1] = __uint_as_float(r.x & 0xFFFF0000u);
-  f[2] = __uint_as_float(r.y << 16); f[3] = __uint_as_float(r.y & 0xFFFF0000u);
-  f[4] = __uint_as_float(r.z << 16); f[5] = __uint_as_float(r.z & 0xFFFF0000u);
-  f[6] = __uint_as_float(r.w << 16); f[7] = __uint_as_float(r.w & 0xFFFF0000u);
-}
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  __nv_bfloat162 t = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&t);
-}
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 o;
-  o.x = pack2(f[0], f[1]); o.y = pack2(f[2], f[3]); o.z = pack2(f[4], f[5]); o.w = pack2(f[6], f[7]);
-  return o;
-}
+static constexpr int kChunkC = 2048;  // channels handled per block of the stats / backward kernels
 
-static constexpr int kChunkC = 2048;  // channels handled per blockIdx.y
+// Thread layout of the stats / backward kernels over one chunk of kChunkC channels: thread threadIdx.x owns the 8-channel
+// group g of the chunk and the pixel rows prow, prow + nrows, ... of the block's pixel range (threads with prow >= nrows idle).
+struct ChanGroups {
+  int c_base, cc;      // first channel of the chunk, channels in it
+  int g, prow, nrows;
+};
+__device__ __forceinline__ ChanGroups chan_groups(int C, int chunk) {
+  ChanGroups t;
+  t.c_base = chunk * kChunkC;
+  t.cc = min(C - t.c_base, kChunkC);
+  const int VG = t.cc >> 3;
+  const int VGb = VG < 256 ? VG : 256;
+  t.nrows = 256 / VGb;
+  t.g = threadIdx.x % VGb;
+  t.prow = threadIdx.x / VGb;
+  return t;
+}
 
 // ---------------------------------------------------------------------------------------------- stats
 __global__ void __launch_bounds__(256) bn_stats_kernel(const bf16* __restrict__ x, long long npix, int C, long long cstride,
@@ -34,14 +37,9 @@ __global__ void __launch_bounds__(256) bn_stats_kernel(const bf16* __restrict__ 
                                                         long long pix_per_block) {
   __shared__ float s_sum[kChunkC];
   __shared__ float s_sq[kChunkC];
-  const int c_base = blockIdx.y * kChunkC;
-  const int cc = min(C - c_base, kChunkC);
-  const int VG = cc >> 3;
+  const auto [c_base, cc, g, prow, nrows] = chan_groups(C, blockIdx.y);
   for (int i = threadIdx.x; i < cc; i += 256) { s_sum[i] = 0.f; s_sq[i] = 0.f; }
   __syncthreads();
-  const int VGb = VG < 256 ? VG : 256;
-  const int nrows = 256 / VGb;
-  const int g = threadIdx.x % VGb, prow = threadIdx.x / VGb;
   if (prow < nrows) {
     float a[8], q[8];
 #pragma unroll
@@ -144,61 +142,81 @@ __global__ void __launch_bounds__(256) scale_shift_act_kernel(const bf16* __rest
     if (!up2) {
       reinterpret_cast<uint4*>(y + p * y_cstride)[g] = o;
     } else {
-      const int hw = (int)(p % ((long long)H * W));
-      const int h = hw / W, w = hw % W;
-      const long long q = ((long long)b * (2 * H) + 2 * h) * (2 * W) + 2 * w;
-      reinterpret_cast<uint4*>(y + q * y_cstride)[g] = o;
-      reinterpret_cast<uint4*>(y + (q + 1) * y_cstride)[g] = o;
-      reinterpret_cast<uint4*>(y + (q + 2 * W) * y_cstride)[g] = o;
-      reinterpret_cast<uint4*>(y + (q + 2 * W + 1) * y_cstride)[g] = o;
+      long long qs[4];
+      quad2x2(p, (int)(p % W), W, qs);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) reinterpret_cast<uint4*>(y + qs[k] * y_cstride)[g] = o;
     }
   }
 }
 
 // ---------------------------------------------------------------------------------------------- backward
-__device__ __forceinline__ void load_dz(const bf16* __restrict__ dy, long long dy_cstride, int b, int h, int w, int H, int W,
-                                        int g, int up2, long long p, float (&dz)[8]) {
-  if (!up2) {
-    unpack8(__ldg(reinterpret_cast<const uint4*>(dy + p * dy_cstride) + g), dz);
+// The backward kernels run one template instance per value of UP2: whether the forward upsampled its output (nearest x2),
+// so that the gradient dy is [B][2H][2W] and dz of a pixel is the sum of dy over its 2x2 block.  A thread owns one 8-channel
+// group of one image; a step of its pixel loop covers U pixels (4, or 2 with UP2, which reads 4 dy vectors per pixel) and
+// issues all of their 16-byte loads before the normalisation arithmetic (only the UP2 dz sums run as the vectors arrive):
+// the kernels are pure streams and their speed is the number of bytes each SM keeps in flight.
+
+// dz of 8 channels as a step holds it until its arithmetic, in the fewer registers: the packed dy vector (4), or with UP2
+// the float sum of the four dy vectors of the 2x2 block (8, not 16).
+template <bool UP2>
+using DzRegs = std::conditional_t<UP2, float[8], uint4>;
+
+// dz of 8 channels (group g) of pixel p = b * H * W + hw, x = hw % W.
+template <bool UP2>
+__device__ __forceinline__ void load_dz(const bf16* __restrict__ dy, long long dy_cstride, long long p, int x, int W, int g,
+                                        DzRegs<UP2>& dz) {
+  if constexpr (!UP2) {
+    dz = __ldg(reinterpret_cast<const uint4*>(dy + p * dy_cstride) + g);
   } else {
-    const long long q = ((long long)b * (2 * H) + 2 * h) * (2 * W) + 2 * w;
-    float t[8];
-    unpack8(__ldg(reinterpret_cast<const uint4*>(dy + q * dy_cstride) + g), dz);
-    unpack8(__ldg(reinterpret_cast<const uint4*>(dy + (q + 1) * dy_cstride) + g), t);
+    long long qs[4];
+    quad2x2(p, x, W, qs);
+    unpack8(__ldg(reinterpret_cast<const uint4*>(dy + qs[0] * dy_cstride) + g), dz);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) dz[j] += t[j];
-    unpack8(__ldg(reinterpret_cast<const uint4*>(dy + (q + 2 * W) * dy_cstride) + g), t);
+    for (int k = 1; k < 4; ++k) {
+      float t[8];
+      unpack8(__ldg(reinterpret_cast<const uint4*>(dy + qs[k] * dy_cstride) + g), t);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) dz[j] += t[j];
-    unpack8(__ldg(reinterpret_cast<const uint4*>(dy + (q + 2 * W + 1) * dy_cstride) + g), t);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) dz[j] += t[j];
+      for (int j = 0; j < 8; ++j) dz[j] += t[j];
+    }
   }
 }
 
-// grid = (pixel chunks, B, channel chunks).  s1[b,c] += sum dz, s2[b,c] += sum dz*xhat; S1[c] += g1[b,c]*part etc.
+// Gradient at the normalised pre-activation z = x * sc + sh of 8 channels: dz, or 0 where a ReLU followed and z <= 0.
+template <bool UP2>
+__device__ __forceinline__ void relu_grad8(const float (&xv)[8], const DzRegs<UP2>& dz, const float (&sc)[8],
+                                           const float (&sh)[8], int relu, float (&d)[8]) {
+  float f[8];
+  if constexpr (UP2) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) f[j] = dz[j];
+  } else {
+    unpack8(dz, f);
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float z = fmaf(xv[j], sc[j], sh[j]);
+    d[j] = (relu && !(z > 0.f)) ? 0.f : f[j];
+  }
+}
+
+// grid = (pixel chunks, B, channel chunks).  s1[b,c] += sum dz, s2[b,c] += sum dz*xhat (bn_bwd_total_kernel forms S1, S2).
+template <bool UP2>
 __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const bf16* __restrict__ dy, long long dy_cstride,
                                                              const bf16* __restrict__ x, long long x_cstride, int H, int W, int C,
                                                              const float* __restrict__ scale, const float* __restrict__ shift,
                                                              int bstride, const float* __restrict__ mean,
-                                                             const float* __restrict__ rstd, int relu, int up2,
-                                                             float* __restrict__ s1, float* __restrict__ s2,
-                                                             float* __restrict__ S1, float* __restrict__ S2, int pix_per_block) {
+                                                             const float* __restrict__ rstd, int relu, float* __restrict__ s1,
+                                                             float* __restrict__ s2, int pix_per_block) {
   __shared__ float a1[kChunkC];
   __shared__ float a2[kChunkC];
   const int b = blockIdx.y;
-  const int c_base = blockIdx.z * kChunkC;
-  const int cc = min(C - c_base, kChunkC);
-  const int VG = cc >> 3;
+  const auto [c_base, cc, g, prow, nrows] = chan_groups(C, blockIdx.z);
   for (int i = threadIdx.x; i < cc; i += 256) { a1[i] = 0.f; a2[i] = 0.f; }
   __syncthreads();
-  const int VGb = VG < 256 ? VG : 256;
-  const int nrows = 256 / VGb;
-  const int g = threadIdx.x % VGb, prow = threadIdx.x / VGb;
   if (prow < nrows) {
     // t2 accumulates sum(d * x) with the RAW input; sum(d * xhat) = rstd * (t2 - mean * t1) is formed once at the end, so the
-    // loop carries no per-channel mean / rstd.  Loads are issued packed (4 registers per 16 bytes) for several pixels before
-    // any arithmetic: the kernel is a pure stream and its speed is the number of bytes each SM keeps in flight.
+    // loop carries no per-channel mean / rstd.
     float t1[8], t2[8], sc[8], sh[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -209,59 +227,29 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const bf16* __restri
     const int HW = H * W;
     const int p0 = blockIdx.x * pix_per_block, p1 = min(p0 + pix_per_block, HW);
     const int gg = (c_base >> 3) + g;
-    if (!up2) {
-      constexpr int U = 4;
-      for (int hw = p0 + prow; hw < p1; hw += U * nrows) {
-        uint4 rx[U], rd[U];
+    constexpr int U = UP2 ? 2 : 4;
+    for (int hw = p0 + prow; hw < p1; hw += U * nrows) {
+      uint4 rx[U];
+      DzRegs<UP2> dz[U];
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const int h2 = hw + u * nrows;
-          if (h2 < p1) {
-            const long long p = (long long)b * HW + h2;
-            rx[u] = __ldg(reinterpret_cast<const uint4*>(x + p * x_cstride) + gg);
-            rd[u] = __ldg(reinterpret_cast<const uint4*>(dy + p * dy_cstride) + gg);
-          }
-        }
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          if (hw + u * nrows < p1) {
-            float xv[8], dz[8];
-            unpack8(rx[u], xv);
-            unpack8(rd[u], dz);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float z = fmaf(xv[j], sc[j], sh[j]);
-              const float d = (relu && !(z > 0.f)) ? 0.f : dz[j];
-              t1[j] += d;
-              t2[j] = fmaf(d, xv[j], t2[j]);
-            }
-          }
+      for (int u = 0; u < U; ++u) {
+        const int h2 = hw + u * nrows;
+        if (h2 < p1) {
+          const long long p = (long long)b * HW + h2;
+          rx[u] = __ldg(reinterpret_cast<const uint4*>(x + p * x_cstride) + gg);
+          load_dz<UP2>(dy, dy_cstride, p, h2 % W, W, gg, dz[u]);
         }
       }
-    } else {
-      for (int hw = p0 + prow; hw < p1; hw += 2 * nrows) {
-        const int hw2 = hw + nrows;
-        const bool two = hw2 < p1;
-        const long long p = (long long)b * HW + hw, q = (long long)b * HW + hw2;
-        float xv[8], dz[8], xw[8], dw[8];
-        unpack8(__ldg(reinterpret_cast<const uint4*>(x + p * x_cstride) + gg), xv);
-        if (two) unpack8(__ldg(reinterpret_cast<const uint4*>(x + q * x_cstride) + gg), xw);
-        load_dz(dy, dy_cstride, b, hw / W, hw % W, H, W, gg, 1, p, dz);
-        if (two) load_dz(dy, dy_cstride, b, hw2 / W, hw2 % W, H, W, gg, 1, q, dw);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float z = fmaf(xv[j], sc[j], sh[j]);
-          const float d = (relu && !(z > 0.f)) ? 0.f : dz[j];
-          t1[j] += d;
-          t2[j] = fmaf(d, xv[j], t2[j]);
-        }
-        if (two) {
+      for (int u = 0; u < U; ++u) {
+        if (hw + u * nrows < p1) {
+          float xv[8], d[8];
+          unpack8(rx[u], xv);
+          relu_grad8<UP2>(xv, dz[u], sc, sh, relu, d);
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
-            const float z = fmaf(xw[j], sc[j], sh[j]);
-            const float d = (relu && !(z > 0.f)) ? 0.f : dw[j];
-            t1[j] += d;
-            t2[j] = fmaf(d, xw[j], t2[j]);
+            t1[j] += d[j];
+            t2[j] = fmaf(d[j], xv[j], t2[j]);
           }
         }
       }
@@ -299,10 +287,8 @@ __global__ void __launch_bounds__(256) bn_bwd_total_kernel(const float* __restri
     a1 = fmaf(g1, s1[(size_t)b * C + c], a1);
     a2 = fmaf(g1, s2[(size_t)b * C + c], a2);
   }
-  for (int o = 16; o > 0; o >>= 1) {
-    a1 += __shfl_xor_sync(0xffffffffu, a1, o);
-    a2 += __shfl_xor_sync(0xffffffffu, a2, o);
-  }
+  a1 = warp_sum(a1);
+  a2 = warp_sum(a2);
   if (lane == 0) {
     S1[c] = a1;
     S2[c] = a2;
@@ -312,25 +298,20 @@ __global__ void __launch_bounds__(256) bn_bwd_total_kernel(const float* __restri
 // dx = scale[b,c]*dz - rstd*(S1/N) - rstd*(S2/N)*xhat   (train) ;   dx = scale[b,c]*dz   (eval: use_batch_stats = 0)
 // grid = (pixel chunks, B, channel chunks) like the reduce kernel: a thread owns one 8-channel group of one image, so
 // every per-(image, channel) constant lives in registers and the loop body is two 16-byte loads, 8 FMAs and one store.
+template <bool UP2>
 __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const bf16* __restrict__ dy, long long dy_cstride,
                                                             const bf16* __restrict__ x, long long x_cstride, int H, int W,
                                                             int C, const float* __restrict__ scale, const float* __restrict__ shift,
                                                             int bstride, const float* __restrict__ mean,
                                                             const float* __restrict__ rstd, const float* __restrict__ S1,
-                                                            const float* __restrict__ S2, float inv_count, int relu, int up2,
+                                                            const float* __restrict__ S2, float inv_count, int relu,
                                                             int use_batch_stats, bf16* __restrict__ dx, long long dx_cstride,
                                                             int pix_per_block) {
   const int b = blockIdx.y;
-  const int c_base = blockIdx.z * kChunkC;
-  const int cc = min(C - c_base, kChunkC);
-  const int VG = cc >> 3;
-  const int VGb = VG < 256 ? VG : 256;
-  const int nrows = 256 / VGb;
-  const int g = threadIdx.x % VGb, prow = threadIdx.x / VGb;
+  const auto [c_base, cc, g, prow, nrows] = chan_groups(C, blockIdx.z);
   if (prow >= nrows) return;
   const int gg = (c_base >> 3) + g;
-  // dx = sc*d - ka - kb*(x - mu) = sc*d - k0 - kb*x with k0 = ka - kb*mu: four constants per channel, loads packed and issued
-  // for several pixels before any arithmetic (see the reduce kernel).
+  // dx = sc*d - ka - kb*(x - mu) = sc*d - k0 - kb*x with k0 = ka - kb*mu: four constants per channel.
   float sc[8], sh[8], k0[8], kb[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
@@ -346,61 +327,29 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const bf16* __restric
   }
   const int HW = H * W;
   const int p0 = blockIdx.x * pix_per_block, p1 = min(p0 + pix_per_block, HW);
-  if (!up2) {
-    constexpr int U = 4;
-    for (int hw = p0 + prow; hw < p1; hw += U * nrows) {
-      uint4 rx[U], rd[U];
+  constexpr int U = UP2 ? 2 : 4;
+  for (int hw = p0 + prow; hw < p1; hw += U * nrows) {
+    uint4 rx[U];
+    DzRegs<UP2> dz[U];
 #pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int h2 = hw + u * nrows;
-        if (h2 < p1) {
-          const long long p = (long long)b * HW + h2;
-          rx[u] = __ldg(reinterpret_cast<const uint4*>(x + p * x_cstride) + gg);
-          rd[u] = __ldg(reinterpret_cast<const uint4*>(dy + p * dy_cstride) + gg);
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int h2 = hw + u * nrows;
-        if (h2 < p1) {
-          float xv[8], dz[8], o[8];
-          unpack8(rx[u], xv);
-          unpack8(rd[u], dz);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float z = fmaf(xv[j], sc[j], sh[j]);
-            const float d = (relu && !(z > 0.f)) ? 0.f : dz[j];
-            o[j] = sc[j] * d - k0[j] - kb[j] * xv[j];
-          }
-          reinterpret_cast<uint4*>(dx + ((long long)b * HW + h2) * dx_cstride)[gg] = pack8(o);
-        }
+    for (int u = 0; u < U; ++u) {
+      const int h2 = hw + u * nrows;
+      if (h2 < p1) {
+        const long long p = (long long)b * HW + h2;
+        rx[u] = __ldg(reinterpret_cast<const uint4*>(x + p * x_cstride) + gg);
+        load_dz<UP2>(dy, dy_cstride, p, h2 % W, W, gg, dz[u]);
       }
     }
-  } else {
-    for (int hw = p0 + prow; hw < p1; hw += 2 * nrows) {
-      const int hw2 = hw + nrows;
-      const bool two = hw2 < p1;
-      const long long pa = (long long)b * HW + hw, pb = (long long)b * HW + hw2;
-      float xa[8], xb[8], da[8], db[8], o[8];
-      unpack8(__ldg(reinterpret_cast<const uint4*>(x + pa * x_cstride) + gg), xa);
-      if (two) unpack8(__ldg(reinterpret_cast<const uint4*>(x + pb * x_cstride) + gg), xb);
-      load_dz(dy, dy_cstride, b, hw / W, hw % W, H, W, gg, 1, pa, da);
-      if (two) load_dz(dy, dy_cstride, b, hw2 / W, hw2 % W, H, W, gg, 1, pb, db);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float z = fmaf(xa[j], sc[j], sh[j]);
-        const float d = (relu && !(z > 0.f)) ? 0.f : da[j];
-        o[j] = sc[j] * d - k0[j] - kb[j] * xa[j];
-      }
-      reinterpret_cast<uint4*>(dx + pa * dx_cstride)[gg] = pack8(o);
-      if (two) {
+    for (int u = 0; u < U; ++u) {
+      const int h2 = hw + u * nrows;
+      if (h2 < p1) {
+        float xv[8], d[8], o[8];
+        unpack8(rx[u], xv);
+        relu_grad8<UP2>(xv, dz[u], sc, sh, relu, d);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float z = fmaf(xb[j], sc[j], sh[j]);
-          const float d = (relu && !(z > 0.f)) ? 0.f : db[j];
-          o[j] = sc[j] * d - k0[j] - kb[j] * xb[j];
-        }
-        reinterpret_cast<uint4*>(dx + pb * dx_cstride)[gg] = pack8(o);
+        for (int j = 0; j < 8; ++j) o[j] = sc[j] * d[j] - k0[j] - kb[j] * xv[j];
+        reinterpret_cast<uint4*>(dx + ((long long)b * HW + h2) * dx_cstride)[gg] = pack8(o);
       }
     }
   }
@@ -509,14 +458,6 @@ __global__ void __launch_bounds__(256) bn_tan_bwd_apply_kernel(const bf16* __res
 
 using namespace sgb;
 
-static inline int ew_blocks(long long total_threads) {
-  long long b = (total_threads + 255) / 256;
-  const long long cap = 16LL * sm_count();
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (int)b;
-}
-
 extern "C" int sgb_bn_stats(const void* x, int64_t npix, int32_t C, int64_t x_cstride, float* sum, float* sumsq,
                             sgb_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
@@ -591,8 +532,9 @@ extern "C" int sgb_bn_bwd_reduce(const void* dy, int64_t dy_cstride, const void*
   int ppb = (int)((HW + target - 1) / target);
   if (ppb < 32) ppb = 32;
   dim3 grid((HW + ppb - 1) / ppb, B, chunks);
-  bn_bwd_reduce_kernel<<<grid, 256, 0, stream>>>((const bf16*)dy, dy_cstride, (const bf16*)x, x_cstride, H, W, C, scale, shift,
-                                                per_image ? C : 0, mean, rstd, relu, up2, s1, s2, S1, S2, ppb);
+  (up2 ? bn_bwd_reduce_kernel<true> : bn_bwd_reduce_kernel<false>)<<<grid, 256, 0, stream>>>(
+      (const bf16*)dy, dy_cstride, (const bf16*)x, x_cstride, H, W, C, scale, shift, per_image ? C : 0, mean, rstd, relu, s1, s2,
+      ppb);
   SGB_LAUNCH_CHECK();
   bn_bwd_total_kernel<<<(C + 7) / 8, 256, 0, stream>>>(s1, s2, scale, per_image ? C : 0, rstd, B, C, S1, S2);
   SGB_LAUNCH_CHECK();
@@ -615,9 +557,9 @@ extern "C" int sgb_bn_bwd_apply(const void* dy, int64_t dy_cstride, const void* 
   int ppb = (int)((HW + target - 1) / target);
   if (ppb < 64) ppb = 64;
   dim3 grid((HW + ppb - 1) / ppb, B, chunks);
-  bn_bwd_apply_kernel<<<grid, 256, 0, stream>>>((const bf16*)dy, dy_cstride, (const bf16*)x, x_cstride, H, W, C, scale, shift,
-                                               per_image ? C : 0, mean, rstd, S1, S2, use_batch_stats ? 1.f / count : 0.f, relu,
-                                               up2, use_batch_stats, (bf16*)dx, dx_cstride, ppb);
+  (up2 ? bn_bwd_apply_kernel<true> : bn_bwd_apply_kernel<false>)<<<grid, 256, 0, stream>>>(
+      (const bf16*)dy, dy_cstride, (const bf16*)x, x_cstride, H, W, C, scale, shift, per_image ? C : 0, mean, rstd, S1, S2,
+      use_batch_stats ? 1.f / count : 0.f, relu, use_batch_stats, (bf16*)dx, dx_cstride, ppb);
   SGB_LAUNCH_CHECK();
   return SGB_OK;
 }

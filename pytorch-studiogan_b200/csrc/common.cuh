@@ -1,6 +1,7 @@
-// Host-side helpers shared by every translation unit of libsgb200: error codes, launch checks,
-// TMA tensor-map encoding resolved through the runtime (no link-time libcuda dependency, so the
-// library also loads on a GPU-less box for the C-ABI export test).
+// Helpers shared by every translation unit of libsgb200.  Host side: error codes, launch checks, the grid size of the
+// grid-stride kernels, TMA tensor-map encoding resolved through the runtime (no link-time libcuda dependency, so the
+// library also loads on a GPU-less box for the C-ABI export test).  Device side: the packed bf16 pair / 16-byte vector
+// format, warp reductions, and the 2x2 block of a nearest x2 upsample / 2x2 pool.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -108,6 +109,54 @@ inline int sm_count() {
   if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   return n;
+}
+
+// Blocks of 256 threads for a grid-stride kernel over total_threads work items: one per 256 items, at most 16 per SM.
+inline int ew_blocks(long long total_threads) {
+  long long b = (total_threads + 255) / 256;
+  const long long cap = 16LL * sm_count();
+  if (b > cap) b = cap;
+  if (b < 1) b = 1;
+  return (int)b;
+}
+
+// A bf16 pair in one 32-bit word, the first element in the low half.
+__device__ __forceinline__ float bf16_bits_lo(uint32_t u) { return __uint_as_float(u << 16); }
+__device__ __forceinline__ float bf16_bits_hi(uint32_t u) { return __uint_as_float(u & 0xFFFF0000u); }
+__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
+  __nv_bfloat162 t = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&t);
+}
+
+// 8 consecutive bf16 channels in one 16-byte vector (the streaming kernels' unit of access).
+__device__ __forceinline__ void unpack8(const uint4& r, float (&f)[8]) {
+  f[0] = bf16_bits_lo(r.x); f[1] = bf16_bits_hi(r.x);
+  f[2] = bf16_bits_lo(r.y); f[3] = bf16_bits_hi(r.y);
+  f[4] = bf16_bits_lo(r.z); f[5] = bf16_bits_hi(r.z);
+  f[6] = bf16_bits_lo(r.w); f[7] = bf16_bits_hi(r.w);
+}
+__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
+  return make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
+}
+
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// Pixel p = (b * h + y) * w + x of a [B][h][w] grid covers the 2x2 block {q, q + 1, q + 2w, q + 2w + 1} of the [B][2h][2w]
+// grid, q = (b * 2h + 2y) * 2w + 2x = 4p - 2x (nearest x2 upsample, 2x2 pooling).  x = p % w is the caller's.
+__device__ __forceinline__ void quad2x2(long long p, int x, int w, long long (&q)[4]) {
+  q[0] = 4 * p - 2 * x;
+  q[1] = q[0] + 1;
+  q[2] = q[0] + 2 * w;
+  q[3] = q[0] + 2 * w + 1;
 }
 
 }  // namespace sgb

@@ -93,13 +93,6 @@ struct EpiOps {
         full_c(F >= 0 && (F & kEpiFull) != 0) {}
 };
 
-__device__ __forceinline__ float bf16_bits_lo(uint32_t u) { return __uint_as_float(u << 16); }
-__device__ __forceinline__ float bf16_bits_hi(uint32_t u) { return __uint_as_float(u & 0xFFFF0000u); }
-__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
-  __nv_bfloat162 t = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&t);
-}
-
 // The arithmetic that follows acc * alpha, for two adjacent channels (c, c + 1): + bias, fmaf(residual, rs, .), ReLU, mask,
 // fmaf(post-mask residual, rs, .).  res / msk: the packed bf16 residual / mask pair (low half = channel c); mbits: the pair's
 // two mask bits (bit plane).  pos: bit 0 / 1 set iff the ReLU output of channel c / c + 1 is positive.

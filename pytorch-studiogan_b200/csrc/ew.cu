@@ -6,32 +6,6 @@
 
 namespace sgb {
 
-__device__ __forceinline__ void unpack8(const uint4& r, float (&f)[8]) {
-  f[0] = __uint_as_float(r.x << 16); f[1] = __uint_as_float(r.x & 0xFFFF0000u);
-  f[2] = __uint_as_float(r.y << 16); f[3] = __uint_as_float(r.y & 0xFFFF0000u);
-  f[4] = __uint_as_float(r.z << 16); f[5] = __uint_as_float(r.z & 0xFFFF0000u);
-  f[6] = __uint_as_float(r.w << 16); f[7] = __uint_as_float(r.w & 0xFFFF0000u);
-}
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  __nv_bfloat162 t = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&t);
-}
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 o;
-  o.x = pack2(f[0], f[1]); o.y = pack2(f[2], f[3]); o.z = pack2(f[4], f[5]); o.w = pack2(f[6], f[7]);
-  return o;
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
 // out = act(a*x + b*y) over [npix][C] with per-tensor channel strides; a may come from a device scalar.
 // act: 0 none, 1 relu.  y may be null (b ignored).  mask (optional): out = mask > 0 ? out : 0.
 __global__ void __launch_bounds__(256) axpby_kernel(const bf16* __restrict__ x, long long xs, const bf16* __restrict__ y,
@@ -76,17 +50,15 @@ __global__ void __launch_bounds__(256) pool2_fwd_kernel(const bf16* __restrict__
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
     const int g = (int)(i % VG);
     const long long p = i / VG;
-    const int wo = (int)(p % Wo), ho = (int)((p / Wo) % Ho), b = (int)(p / ((long long)Wo * Ho));
-    const long long q = ((long long)b * (2 * Ho) + 2 * ho) * (2 * Wo) + 2 * wo;
-    float f0[8], f1[8], f2[8], f3[8], o[8];
-    unpack8(__ldg(reinterpret_cast<const uint4*>(x + q * xs) + g), f0);
-    unpack8(__ldg(reinterpret_cast<const uint4*>(x + (q + 1) * xs) + g), f1);
-    unpack8(__ldg(reinterpret_cast<const uint4*>(x + (q + 2 * Wo) * xs) + g), f2);
-    unpack8(__ldg(reinterpret_cast<const uint4*>(x + (q + 2 * Wo + 1) * xs) + g), f3);
+    long long qs[4];
+    quad2x2(p, (int)(p % Wo), Wo, qs);
+    float f[4][8], o[8];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) unpack8(__ldg(reinterpret_cast<const uint4*>(x + qs[k] * xs) + g), f[k]);
 #pragma unroll
     for (int j = 0; j < 8; ++j)
-      o[j] = mode == 1 ? fmaxf(fmaxf(f0[j], f1[j]), fmaxf(f2[j], f3[j]))
-                       : (mode == 0 ? 0.25f : 1.0f) * (f0[j] + f1[j] + f2[j] + f3[j]);  // 0 average, 2 sum
+      o[j] = mode == 1 ? fmaxf(fmaxf(f[0][j], f[1][j]), fmaxf(f[2][j], f[3][j]))
+                       : (mode == 0 ? 0.25f : 1.0f) * (f[0][j] + f[1][j] + f[2][j] + f[3][j]);  // 0 average, 2 sum
     reinterpret_cast<uint4*>(y + p * ys)[g] = pack8(o);
   }
 }
@@ -101,9 +73,8 @@ __global__ void __launch_bounds__(256) relu_pool2_kernel(const bf16* __restrict_
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
     const int g = (int)(i % VG);
     const long long p = i / VG;
-    const int wo = (int)(p % Wo), ho = (int)((p / Wo) % Ho), b = (int)(p / ((long long)Wo * Ho));
-    const long long q = ((long long)b * (2 * Ho) + 2 * ho) * (2 * Wo) + 2 * wo;
-    const long long qs[4] = {q, q + 1, q + 2 * Wo, q + 2 * Wo + 1};
+    long long qs[4];
+    quad2x2(p, (int)(p % Wo), Wo, qs);
     float f[4][8], o[8];
 #pragma unroll
     for (int k = 0; k < 4; ++k) unpack8(__ldg(reinterpret_cast<const uint4*>(x + qs[k] * xs) + g), f[k]);
@@ -132,9 +103,8 @@ __global__ void __launch_bounds__(256) pool2_bwd_kernel(const bf16* __restrict__
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
     const int g = (int)(i % VG);
     const long long p = i / VG;
-    const int wo = (int)(p % Wo), ho = (int)((p / Wo) % Ho), b = (int)(p / ((long long)Wo * Ho));
-    const long long q0 = ((long long)b * (2 * Ho) + 2 * ho) * (2 * Wo) + 2 * wo;
-    const long long qs[4] = {q0, q0 + 1, q0 + 2 * Wo, q0 + 2 * Wo + 1};
+    long long qs[4];
+    quad2x2(p, (int)(p % Wo), Wo, qs);
     float d[8];
     unpack8(__ldg(reinterpret_cast<const uint4*>(dy + p * dys) + g), d);
     float o[4][8];
@@ -213,8 +183,8 @@ __global__ void __launch_bounds__(256) dhead_fwd_kernel(const float* __restrict_
     a1 = fmaf(hv, __ldg(w1 + c), a1);
     if (ep) a2 = fmaf(hv, __ldg(ep + c), a2);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) { a1 += __shfl_xor_sync(0xffffffffu, a1, o); a2 += __shfl_xor_sync(0xffffffffu, a2, o); }
+  a1 = warp_sum(a1);
+  a2 = warp_sum(a2);
   if (lane == 0) {
     float r = sigma1 ? a1 / __ldg(sigma1) : a1;
     if (b1) r += __ldg(b1);
@@ -274,8 +244,7 @@ __global__ void __launch_bounds__(256) rowdot_kernel(const bf16* __restrict__ x,
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc = fmaf(a[j], b[j], acc);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  acc = warp_sum(acc);
   if (lane == 0) out[row] = acc;
 }
 
@@ -474,7 +443,7 @@ __global__ void __launch_bounds__(256) col27_kernel(const void* __restrict__ src
   const long long total = (long long)B * H * W;
   for (long long p = (long long)blockIdx.x * 256 + threadIdx.x; p < total; p += (long long)gridDim.x * 256) {
     const int w = (int)(p % W), h = (int)((p / W) % H), b = (int)(p / ((long long)W * H));
-    float v[32];
+    float v[4][8];                                   // k = t * 3 + c at v[k / 8][k % 8]
 #pragma unroll
     for (int t = 0; t < 9; ++t) {
       const int hh = h + t / 3 - 1, ww = w + t % 3 - 1;
@@ -486,19 +455,13 @@ __global__ void __launch_bounds__(256) col27_kernel(const void* __restrict__ src
           if (src_nchw) x = __ldg(reinterpret_cast<const float*>(src) + (((long long)b * 3 + c) * H + hh) * W + ww);
           else x = __bfloat162float(reinterpret_cast<const bf16*>(src)[(((long long)b * H + hh) * W + ww) * cs + c]);
         }
-        v[t * 3 + c] = x;
+        v[(t * 3 + c) / 8][(t * 3 + c) % 8] = x;
       }
     }
 #pragma unroll
-    for (int k = 27; k < 32; ++k) v[k] = 0.f;
-    uint4* op = reinterpret_cast<uint4*>(out + p * 32);
+    for (int k = 27; k < 32; ++k) v[3][k - 24] = 0.f;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      uint4 o;
-      o.x = pack2(v[8 * j + 0], v[8 * j + 1]); o.y = pack2(v[8 * j + 2], v[8 * j + 3]);
-      o.z = pack2(v[8 * j + 4], v[8 * j + 5]); o.w = pack2(v[8 * j + 6], v[8 * j + 7]);
-      op[j] = o;
-    }
+    for (int j = 0; j < 4; ++j) reinterpret_cast<uint4*>(out + p * 32)[j] = pack8(v[j]);
   }
 }
 
@@ -645,7 +608,7 @@ __global__ void __launch_bounds__(256) resize_norm_kernel(const float* __restric
     const long long total = (long long)B * So * So;
     for (long long p = (long long)blockIdx.x * 256 + threadIdx.x; p < total; p += (long long)gridDim.x * 256) {
       const int wo = (int)(p % So), ho = (int)((p / So) % So), b = (int)(p / ((long long)So * So));
-      float v[32];
+      float v[4][8];                                 // k = t * 3 + c at v[k / 8][k % 8], as in col27_kernel
 #pragma unroll
       for (int t = 0; t < 9; ++t)
 #pragma unroll
@@ -653,18 +616,12 @@ __global__ void __launch_bounds__(256) resize_norm_kernel(const float* __restric
           const float* src = img + ((long long)b * 3 + c) * H * W;
           const float r = friendly ? resized_pixel_pil(src, quantize, H, W, S, 2 * ho + t / 3, 2 * wo + t % 3)
                                    : resized_pixel(src, quantize, H, W, S, 2 * ho + t / 3, 2 * wo + t % 3, scale_h, scale_w);
-          v[t * 3 + c] = (r / 255.0f - 0.5f) / 0.5f;
+          v[(t * 3 + c) / 8][(t * 3 + c) % 8] = (r / 255.0f - 0.5f) / 0.5f;
         }
 #pragma unroll
-      for (int k = 27; k < 32; ++k) v[k] = 0.f;
-      uint4* op = reinterpret_cast<uint4*>(out_col + p * 32);
+      for (int k = 27; k < 32; ++k) v[3][k - 24] = 0.f;
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        uint4 o;
-        o.x = pack2(v[8 * j + 0], v[8 * j + 1]); o.y = pack2(v[8 * j + 2], v[8 * j + 3]);
-        o.z = pack2(v[8 * j + 4], v[8 * j + 5]); o.w = pack2(v[8 * j + 6], v[8 * j + 7]);
-        op[j] = o;
-      }
+      for (int j = 0; j < 4; ++j) reinterpret_cast<uint4*>(out_col + p * 32)[j] = pack8(v[j]);
     }
   }
 }
@@ -746,7 +703,7 @@ __global__ void __launch_bounds__(256) gp_sumsq_kernel(const float* __restrict__
   float acc = 0.f;
   for (long long i = (long long)k * 256 + threadIdx.x; i < n_per; i += (long long)blocks_per_sample * 256) acc = fmaf(gb[i], gb[i], acc);
   __shared__ float red[8];
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  acc = warp_sum(acc);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -767,14 +724,6 @@ __global__ void __launch_bounds__(256) gp_seed_kernel(const float* __restrict__ 
 }  // namespace sgb
 
 using namespace sgb;
-
-static inline int ew_blocks(long long total_threads) {
-  long long b = (total_threads + 255) / 256;
-  const long long cap = 16LL * sm_count();
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (int)b;
-}
 
 extern "C" int sgb_axpby(const void* x, int64_t xs, const void* y, int64_t ys, const void* mask, int64_t ms, void* out,
                          int64_t os, int64_t npix, int32_t C, float a, const float* a_dev, float b, int32_t act,

@@ -25,12 +25,6 @@ __global__ void __launch_bounds__(256) zero_stuff2_kernel(const bf16* __restrict
   }
 }
 
-static inline int rs_blocks(long long work) {
-  long long b = (work + 255) / 256;
-  const long long cap = 16LL * sm_count();
-  return (int)(b < 1 ? 1 : (b > cap ? cap : b));
-}
-
 }  // namespace sgb
 
 using namespace sgb;
@@ -39,7 +33,7 @@ extern "C" int sgb_zero_stuff2(const void* x, int64_t xs, void* y, int64_t ys, i
                                sgb_stream_t stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   SGB_REQUIRE(x && y && B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && xs % 8 == 0 && ys % 8 == 0);
-  zero_stuff2_kernel<<<rs_blocks((long long)B * 4 * H * W * (C / 8)), 256, 0, stream>>>((const bf16*)x, xs, (bf16*)y, ys, B, H, W, C);
+  zero_stuff2_kernel<<<ew_blocks((long long)B * 4 * H * W * (C / 8)), 256, 0, stream>>>((const bf16*)x, xs, (bf16*)y, ys, B, H, W, C);
   SGB_LAUNCH_CHECK();
   return SGB_OK;
 }

@@ -8,12 +8,6 @@
 
 namespace sgb {
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 __device__ float block_sum(float v, float* sh) {
   v = warp_sum(v);
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
