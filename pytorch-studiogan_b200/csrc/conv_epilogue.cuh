@@ -262,9 +262,8 @@ static constexpr int kEpiThreads = 256;           // 8 epilogue warps
 // consumes its chunks, so their ~1-2 us latency under load overlaps ``depth`` chunks of epilogue work instead of one.
 struct EpiAux {
   int kind;                 // 1 residual, 2 mask
-  uint32_t ring;            // this team's first aux tile (1024-byte aligned), tiles 16 KiB apart
-  uint32_t full0, empty0;   // this team's first full / empty mbarrier (8 bytes apart per slot)
-  int depth;                // ring slots per team
+  uint32_t tiles;           // this team's first aux tile (1024-byte aligned), tiles 16 KiB apart
+  MbarRing ring;            // this team's ring, one slot per tile
   uint32_t* cnt;            // per-thread count of chunks consumed by this team
   int arow;                 // aux-tile row this thread reads
 };
@@ -373,9 +372,8 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
     named_bar_sync(1 + team, kTeamThreads);
     uint32_t arow_addr = 0u, aslot = 0u;
     if (aux_kind) {                              // residual / mask / P chunk: one TMA box (fetched ahead by the aux producer warp)
-      aslot = *aux->cnt % (uint32_t)aux->depth;
-      mbar_wait(aux->full0 + 8u * aslot, (*aux->cnt / (uint32_t)aux->depth) & 1u);
-      arow_addr = aux->ring + aslot * kEpiStageBytes + (uint32_t)aux->arow * 128u;
+      aslot = aux->ring.wait(*aux->cnt);
+      arow_addr = aux->tiles + aslot * kEpiStageBytes + (uint32_t)aux->arow * 128u;
       *aux->cnt += 1u;
     }
     // compile-time variants handle two 16-column pieces per iteration: both accumulator loads are in flight together
@@ -450,7 +448,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
     if (leader) {
       tma_store_4d(tmY, stage_cur, nbase, c1, c2, c3);
       bulk_commit();
-      if (aux_kind) mbar_arrive(aux->empty0 + 8u * aslot);   // every thread of the team is past its last read of the aux tile (barrier above)
+      if (aux_kind) mbar_arrive(aux->ring.empty(aslot));   // every thread of the team is past its last read of the aux tile (barrier above)
     }
   }
 }

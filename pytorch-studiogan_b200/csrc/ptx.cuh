@@ -180,6 +180,66 @@ __device__ __forceinline__ void acc_fence(float (&d)[R]) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// ---------------------------------------------------------------- mbarrier rings
+// A ring of `slots` shared-memory buffers handed from a TMA producer to its consumers, guarded by one block of mbarriers
+// [full x slots][empty x slots].  Both sides count the same running position it: slot it % slots, in round it / slots.
+// A full barrier completes once per round (one producer arrival plus the TMA bytes), an empty barrier once the consumers
+// are done with the slot, so a producer waits with the other parity (a fresh ring counts as released).
+struct MbarRing {
+  uint32_t bar;   // first full barrier
+  int slots;
+  __host__ __device__ static constexpr uint32_t bytes(int slots) { return 16u * (uint32_t)slots; }
+  __host__ __device__ uint32_t end() const { return bar + bytes(slots); }
+  __device__ uint32_t full(int s) const { return bar + 8u * s; }
+  __device__ uint32_t empty(int s) const { return bar + 8u * (slots + s); }
+  __device__ int slot(uint32_t it) const { return it % slots; }
+  __device__ uint32_t phase(uint32_t it) const { return (it / slots) & 1; }
+  // Thread 0, before the CTA-wide barrier that publishes the ring.
+  __device__ void init(uint32_t consumer_arrivals) const {
+    for (int s = 0; s < slots; ++s) {
+      mbar_init(full(s), 1);
+      mbar_init(empty(s), consumer_arrivals);
+    }
+  }
+  // Producer: waits until position it's slot is released, then arms its full barrier for tx_bytes of TMA loads.
+  __device__ int acquire(uint32_t it, uint32_t tx_bytes) const {
+    const int s = slot(it);
+    mbar_wait(empty(s), phase(it) ^ 1);
+    mbar_arrive_expect_tx(full(s), tx_bytes);
+    return s;
+  }
+  // Consumer: waits until position it's slot is filled.
+  __device__ int wait(uint32_t it) const {
+    const int s = slot(it);
+    mbar_wait(full(s), phase(it));
+    return s;
+  }
+  // Consumer warp (converged): one arrival on slot s's empty barrier, from lane 0.
+  __device__ void release(int s) const {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(empty(s));
+  }
+  // Consumer warp, after committing the MMAs that read slot s: once the previous group has retired, its slot (prev) is free.
+  __device__ void release_prev(int& prev, int s) const {
+    wgmma_wait<1>();
+    if (prev >= 0) release(prev);
+    prev = s;
+  }
+};
+
+// Dynamic shared memory is carved from its first 1024-byte boundary (SWIZZLE_128B tiles need it), so the host requests a
+// layout's total plus the worst-case padding.
+__device__ __forceinline__ uint32_t smem_aligned(const void* smem_raw) { return (smem_u32(smem_raw) + 1023u) & ~1023u; }
+inline size_t smem_request(uint32_t total) { return (size_t)total + 1024; }
+
+// The constant B operand of the bias-gradient MMAs: 1 KiB of bf16 1.0 (8 K-major rows of 64), written by a CTA of nthreads and
+// fenced for the tensor cores, which read it through the async proxy.  Precedes the CTA-wide barrier.
+static constexpr uint32_t kOnesSlabBytes = 1024;
+__device__ __forceinline__ void fill_ones_slab(uint32_t base, int nthreads) {
+  for (int i = threadIdx.x; i < (int)kOnesSlabBytes / 4; i += nthreads) st_shared_b32(base + 4u * i, 0x3F803F80u);
+  fence_proxy_async_smem();
+}
+
 // Accumulator staging in shared memory: fp32 rows of ``ld`` = acc_row_bytes(N) bytes, 16 more than the row (the padding
 // staggers consecutive rows across the banks, so the one-row-per-thread 16-byte reads of the fused epilogues do not conflict).
 __host__ __device__ inline uint32_t acc_row_bytes(int N) { return (uint32_t)N * 4u + 16u; }

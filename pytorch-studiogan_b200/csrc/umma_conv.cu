@@ -60,28 +60,55 @@ __device__ __forceinline__ FpropTile fprop_tile(const FpropArgs& p, int t) {
   return c;
 }
 
+__host__ __device__ constexpr bool fprop_is_pingpong(int f) { return f >= 0 && (f & (kEpiSmStats | kEpiSmApply | kEpiSmBwd)) == 0; }
+
+// Shared memory of conv_fprop_kernel: addresses from base, or offsets from the 1024-aligned base when base = 0.  Every tile
+// region is a multiple of 1024 bytes (b_bytes too: BN % 8 == 0).
+struct FpropSmem {
+  uint32_t epi;                   // staging tiles of the two epilogue teams (use_tma)
+  uint32_t aux;                   // aux tiles, aux_depth per team (aux_kind)
+  uint32_t bres;                  // resident weight tiles [tap][kb] (b_resident)
+  uint32_t acc;                   // fp32 accumulator rows of the tile (staged schedule)
+  uint32_t ring;                  // operand ring: stages x (A tile, B tile unless resident)
+  uint32_t stage_bytes, b_bytes;
+  MbarRing ops, bres_ready, aux0; // barriers: operand ring, resident filter (one slot, filled once), team 0's aux ring
+  uint32_t total;
+  __host__ __device__ MbarRing aux_ring(int team) const { return {aux0.bar + MbarRing::bytes(aux0.slots) * team, aux0.slots}; }
+};
+__host__ __device__ inline FpropSmem fprop_smem(const FpropArgs& p, bool pingpong, uint32_t base = 0) {
+  FpropSmem L;
+  L.b_bytes = (uint32_t)p.BN * kBlockK * 2;   // same size for K-major [BN][64] and MN-major (BN/64) x [64][64]
+  L.stage_bytes = kABytes + (p.b_resident ? 0u : L.b_bytes);
+  L.epi = base;
+  L.aux = L.epi + (p.use_tma ? 2u * p.epi_nbuf * (pingpong ? kFragStageBytes : kEpiStageBytes) : 0u);
+  L.bres = L.aux + (p.aux_kind ? 2u * p.aux_depth * kEpiStageBytes : 0u);
+  L.acc = L.bres + (p.b_resident ? (uint32_t)(p.taps * p.kblocks) * L.b_bytes : 0u);
+  L.ring = L.acc + (pingpong ? 0u : (uint32_t)kTileM * acc_row_bytes(p.BN));   // 128 rows x (16 mod 1024) B
+  L.ops = {L.ring + (uint32_t)p.stages * L.stage_bytes, p.stages};
+  L.bres_ready = {L.ops.end(), 1};
+  L.aux0 = {L.bres_ready.end(), p.aux_depth};
+  L.total = L.aux_ring(1).end() - base;
+  return L;
+}
+
 // Main loop of one fprop tile on one consumer warpgroup: per 16-wide K step, M m64 wgmmas against the same B tile, row block h
 // of the A tile at a_off + h * 8 KiB -> acc[h].  it = the tile's first position in the operand ring.
 template <int BN, int M>
-__device__ __forceinline__ void fprop_mma(const FpropArgs& p, float (&acc)[M][BN / 2], uint32_t a_off, uint32_t smem_base,
-                                          uint32_t stage_bytes, uint32_t bres_base, uint32_t b_bytes, uint32_t bar_base, uint32_t it) {
+__device__ __forceinline__ void fprop_mma(const FpropArgs& p, const FpropSmem& L, float (&acc)[M][BN / 2], uint32_t a_off, uint32_t it) {
 #pragma unroll
   for (int h = 0; h < M; ++h)
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
   const bool b_mn = (p.w_mode == 2);
   const int kiters = p.taps * p.kblocks;
-  const uint32_t lane = threadIdx.x & 31;
   int prev = -1;
   for (int k = 0; k < kiters; ++k, ++it) {
-    const int s = it % p.stages;
-    const uint32_t ph = (it / p.stages) & 1;
-    mbar_wait(bar_base + 8u * s, ph);
-    const uint32_t sa = smem_base + s * stage_bytes;
+    const int s = L.ops.wait(it);
+    const uint32_t sa = L.ring + s * L.stage_bytes;
     const uint64_t adesc = make_sdesc_sw128(sa + a_off, 16, 1024);          // [128][64]; row block h is 8 KiB further
     // K-major B: rows = output channels, +32 B per 16-wide K step.
     // MN-major B: (BN/64) atoms of [64 k-rows][64 n] 8 KiB apart (LBO), 8-row groups 1 KiB apart (SBO), +2 KiB per K step.
-    const uint32_t sb = p.b_resident ? bres_base + (uint32_t)k * b_bytes : sa + kABytes;     // k = tap * kblocks + kb
+    const uint32_t sb = p.b_resident ? L.bres + (uint32_t)k * L.b_bytes : sa + kABytes;     // k = tap * kblocks + kb
     wgmma_fence();
     if (b_mn) {
       const uint64_t bdesc = make_sdesc_sw128(sb, 8192, 1024);
@@ -99,33 +126,28 @@ __device__ __forceinline__ void fprop_mma(const FpropArgs& p, float (&acc)[M][BN
           Wgmma<BN>::template mma<0, 0>(acc[h], adesc + 512 * h + 2 * kk, bdesc + 2 * kk, (k > 0 || kk > 0) ? 1u : 0u);
     }
     wgmma_commit();
-    wgmma_wait<1>();                          // the previous K block's MMAs have retired: its ring slot is free
-    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev)); }
-    prev = s;
+    L.ops.release_prev(prev, s);              // the previous K block's MMAs have retired: its ring slot is free
   }
   wgmma_wait<0>();
 #pragma unroll
   for (int h = 0; h < M; ++h) acc_fence(acc[h]);
-  __syncwarp();
-  if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev));
+  L.ops.release(prev);
 }
 
 // Staged schedule: the main loop of this consumer warpgroup's 64 rows (64 wg .. 64 wg + 63) of the tile, then its accumulators
 // -> shared memory.
 template <int BN>
-__device__ __forceinline__ void fprop_staged_mma(const FpropArgs& p, uint32_t smem_base, uint32_t stage_bytes, uint32_t bres_base,
-                                                 uint32_t b_bytes, uint32_t bar_base, uint32_t it, int wg, uint32_t acc_base) {
+__device__ __forceinline__ void fprop_staged_mma(const FpropArgs& p, const FpropSmem& L, uint32_t it, int wg) {
   float acc[1][BN / 2];
-  fprop_mma<BN, 1>(p, acc, (uint32_t)wg * 8192u, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it);
+  fprop_mma<BN, 1>(p, L, acc, (uint32_t)wg * 8192u, it);
   named_bar_sync(kAccBar, kConsumerThreads);  // every consumer is done reading the previous tile's staged accumulators
-  acc_store<BN>(acc[0], acc_base + (uint32_t)wg * 64u * acc_row_bytes(BN), acc_row_bytes(BN));
+  acc_store<BN>(acc[0], L.acc + (uint32_t)wg * 64u * acc_row_bytes(BN), acc_row_bytes(BN));
   named_bar_sync(kAccBar, kConsumerThreads);
 }
 
 // ------------------------------------------------------------------------------------------------ fprop, ping-pong schedule
 // Compile-time epilogue variants other than the softmax ones: each consumer warpgroup owns whole 128-row tiles (local tile i
 // goes to warpgroup i & 1) and runs the epilogue straight from its registers while the other warpgroup issues its MMAs.
-__host__ __device__ constexpr bool fprop_is_pingpong(int f) { return f >= 0 && (f & (kEpiSmStats | kEpiSmApply | kEpiSmBwd)) == 0; }
 static constexpr uint32_t kTurnBar = 4;       // named barriers 4 / 5: warpgroup 0 / 1 may start its next mainloop
 
 // One consumer warpgroup of the ping-pong schedule.  The two warpgroups' main loops take turns (named barriers kTurnBar + wg),
@@ -133,9 +155,7 @@ static constexpr uint32_t kTurnBar = 4;       // named barriers 4 / 5: warpgroup
 // 64-channel chunk through this warpgroup's staging tiles; a residual / mask chunk arrives in this warpgroup's aux ring as one
 // box of the whole tile, read by both halves.
 template <int F, int BN>
-__device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUtensorMap* tmY, uint32_t smem_base, uint32_t stage_bytes,
-                                                  uint32_t bres_base, uint32_t b_bytes, uint32_t bar_base, uint32_t epi_stage_base,
-                                                  uint32_t aux_stage_base, int wg) {
+__device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUtensorMap* tmY, const FpropSmem& L, int wg) {
   constexpr int aux_kind = (F & kEpiAuxRes) ? 1 : ((F & kEpiAuxMask) ? 2 : 0);
   const uint32_t w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const bool leader = (threadIdx.x & 127) == 0;
@@ -155,20 +175,19 @@ __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUte
       arow[h][hr] = aux_half ? (uint32_t)((bi[h][hr] * p.aux_th + (p.aux_th == p.th ? hi[h][hr] : (hi[h][hr] >> 1))) * p.aux_tw + (wi[h][hr] >> 1))
                              : (uint32_t)row;
     }
-  const uint32_t stage = epi_stage_base + (uint32_t)(wg * p.epi_nbuf) * kFragStageBytes;
-  const uint32_t aux_ring = aux_stage_base + (uint32_t)(wg * p.aux_depth) * kEpiStageBytes;
-  const uint32_t aux_full0 = bar_base + 8u * (2 * p.stages + 1 + wg * p.aux_depth);
-  const uint32_t aux_empty0 = bar_base + 8u * (2 * p.stages + 1 + (2 + wg) * p.aux_depth);
+  const uint32_t stage = L.epi + (uint32_t)(wg * p.epi_nbuf) * kFragStageBytes;
+  const uint32_t aux_tiles = L.aux + (uint32_t)(wg * p.aux_depth) * kEpiStageBytes;
+  const MbarRing aux = L.aux_ring(wg);
   const int kiters = p.taps * p.kblocks;
   const int n_local = (p.num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // this CTA's tiles
   uint32_t sbuf = 0, aux_cnt = 0;
-  if (p.b_resident) mbar_wait(bar_base + 8u * (2 * p.stages), 0);
+  if (p.b_resident) L.bres_ready.wait(0);
   for (int i = wg; i < n_local; i += 2) {
     const FpropTile tc = fprop_tile(p, (int)blockIdx.x + i * (int)gridDim.x);
     const int nt = tc.nt, wt = tc.wt, ht = tc.ht, bt = tc.bt;
     float acc[2][BN / 2];
     if (i > 0) named_bar_sync(kTurnBar + wg, 256);          // the other warpgroup has issued tile i - 1
-    fprop_mma<BN, 2>(p, acc, 0u, smem_base, stage_bytes, bres_base, b_bytes, bar_base, (uint32_t)(i * kiters));
+    fprop_mma<BN, 2>(p, L, acc, 0u, (uint32_t)(i * kiters));
     if (i + 1 < n_local) named_bar_arrive(kTurnBar + (wg ^ 1), 256);
     long long pix[2][2], rpix[2][2];
     bool valid[2][2];
@@ -192,9 +211,8 @@ __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUte
       if (nbase >= p.e.Cout) break;                 // (the aux producer skips the same chunks)
       uint32_t aux_tile = 0u, aslot = 0u;
       if constexpr (aux_kind != 0) {
-        aslot = aux_cnt % (uint32_t)p.aux_depth;
-        mbar_wait(aux_full0 + 8u * aslot, (aux_cnt / (uint32_t)p.aux_depth) & 1u);
-        aux_tile = aux_ring + aslot * kEpiStageBytes;
+        aslot = aux.wait(aux_cnt);
+        aux_tile = aux_tiles + aslot * kEpiStageBytes;
         ++aux_cnt;
       }
       epilogue_frag_chunk<F, BN>(p.e, tmY, acc[0], cc, nbase, c1[0], c2[0], c3[0], pix[0], rpix[0], valid[0], alpha, stage,
@@ -202,7 +220,7 @@ __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUte
       epilogue_frag_chunk<F, BN>(p.e, tmY, acc[1], cc, nbase, c1[1], c2[1], c3[1], pix[1], rpix[1], valid[1], alpha, stage,
                                  p.epi_nbuf, sbuf, 1u + wg, leader, aux_tile, arow[1]);
       // every thread of the warpgroup is past its last read of the aux box (the barrier before the second half's store)
-      if (aux_kind != 0 && leader) mbar_arrive(aux_empty0 + 8u * aslot);
+      if (aux_kind != 0 && leader) mbar_arrive(aux.empty(aslot));
     }
   }
   if (leader) bulk_wait_all();                    // staging tiles must outlive the last tensor store
@@ -211,9 +229,7 @@ __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUte
 // Staged-epilogue consumer (run-time flags and softmax variants): both warpgroups run the MMAs of every tile, stage the
 // accumulators in shared memory as fp32 rows, then run the epilogue on them.
 template <int F>
-__device__ __forceinline__ void fprop_staged_consumer(const FpropArgs& p, const CUtensorMap* tmY, uint32_t smem_base, uint32_t stage_bytes,
-                                                      uint32_t bres_base, uint32_t b_bytes, uint32_t bar_base, uint32_t epi_stage_base,
-                                                      uint32_t aux_stage_base, uint32_t acc_base, int wg) {
+__device__ __forceinline__ void fprop_staged_consumer(const FpropArgs& p, const CUtensorMap* tmY, const FpropSmem& L, int wg) {
   // Epilogue: team = which 64-channel chunks (even / odd) = consumer warpgroup, q = which 32 rows.
   const int ct = threadIdx.x - 128;
   const int lane = threadIdx.x & 31;
@@ -224,18 +240,16 @@ __device__ __forceinline__ void fprop_staged_consumer(const FpropArgs& p, const 
   const int wi = row % p.tw, hi = (row / p.tw) % p.th, bi = row / (p.tw * p.th);
   const bool vec_ok = epi_vec_ok(p.e);
   const float alpha = epi_alpha(p.e);
-  const uint32_t stage = epi_stage_base + team * p.epi_nbuf * kEpiStageBytes;
-  const uint32_t t_row = acc_base + (uint32_t)row * acc_row_bytes(p.BN);
+  const uint32_t stage = L.epi + team * p.epi_nbuf * kEpiStageBytes;
+  const uint32_t t_row = L.acc + (uint32_t)row * acc_row_bytes(p.BN);
   const int kiters = p.taps * p.kblocks;
   uint32_t aux_cnt = 0, sbuf = 0, it = 0;
   EpiAux aux;
-  aux.kind = p.aux_kind; aux.ring = aux_stage_base + (uint32_t)(team * p.aux_depth) * kEpiStageBytes;
-  aux.full0 = bar_base + 8u * (2 * p.stages + 1 + team * p.aux_depth);
-  aux.empty0 = bar_base + 8u * (2 * p.stages + 1 + (2 + team) * p.aux_depth);
-  aux.depth = p.aux_depth; aux.cnt = &aux_cnt;
+  aux.kind = p.aux_kind; aux.tiles = L.aux + (uint32_t)(team * p.aux_depth) * kEpiStageBytes;
+  aux.ring = L.aux_ring(team); aux.cnt = &aux_cnt;
   const bool aux_half = p.aux_kind == 1 && p.e.res_up2;
   aux.arow = aux_half ? ((bi * p.aux_th + (p.aux_th == p.th ? hi : (hi >> 1))) * p.aux_tw + (wi >> 1)) : row;
-  if (p.b_resident) mbar_wait(bar_base + 8u * (2 * p.stages), 0);
+  if (p.b_resident) L.bres_ready.wait(0);
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, it += kiters) {
     const FpropTile tc = fprop_tile(p, tile);
     const int nt = tc.nt, wt = tc.wt, ht = tc.ht, bt = tc.bt;
@@ -247,10 +261,10 @@ __device__ __forceinline__ void fprop_staged_consumer(const FpropArgs& p, const 
     const long long rpix = epi_rpix(p.e, b, h, w, p.H, p.W, pix);
 
     switch (p.BN) {
-      case 16: fprop_staged_mma<16>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
-      case 32: fprop_staged_mma<32>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
-      case 64: fprop_staged_mma<64>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
-      default: fprop_staged_mma<128>(p, smem_base, stage_bytes, bres_base, b_bytes, bar_base, it, wg, acc_base); break;
+      case 16: fprop_staged_mma<16>(p, L, it, wg); break;
+      case 32: fprop_staged_mma<32>(p, L, it, wg); break;
+      case 64: fprop_staged_mma<64>(p, L, it, wg); break;
+      default: fprop_staged_mma<128>(p, L, it, wg); break;
     }
     if constexpr (F >= 0 && (F & kEpiSmStats) != 0) {
       epilogue_tile_smstats(p.e, t_row, p.BN, n0, valid, pix, alpha, team, nt * 2 + team);
@@ -270,21 +284,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmAux, const FpropArgs p) {
   constexpr bool pingpong = fprop_is_pingpong(F);
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t epi_stage_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // staging tiles when use_tma
-  const uint32_t epi_bytes = p.use_tma ? 2u * p.epi_nbuf * (pingpong ? kFragStageBytes : kEpiStageBytes) : 0u;
-  const uint32_t aux_stage_base = epi_stage_base + epi_bytes;            // + aux tiles when aux_kind
-  const uint32_t b_bytes = (uint32_t)p.BN * kBlockK * 2;  // same size for K-major [BN][64] and MN-major (BN/64) x [64][64]
-  const uint32_t bres_base = aux_stage_base + (p.aux_kind ? 2u * p.aux_depth * kEpiStageBytes : 0u);     // resident weight tiles [tap][kb]
-  const uint32_t acc_base = bres_base + (p.b_resident ? (uint32_t)(p.taps * p.kblocks) * b_bytes : 0u);  // fp32 accumulator rows
-  // 1024-aligned: 128 rows x (16 mod 1024) B
-  const uint32_t smem_base = acc_base + (pingpong ? 0u : (uint32_t)kTileM * acc_row_bytes(p.BN));
-  const uint32_t stage_bytes = kABytes + (p.b_resident ? 0u : b_bytes);  // multiple of 1024 because BN % 8 == 0 -> b_bytes % 1024 == 0
-  const uint32_t bar_base = smem_base + (uint32_t)p.stages * stage_bytes;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-  const uint32_t bres_bar = bar_base + 8u * (2 * p.stages);
-  auto aux_full = [&](int team, int slot) { return bar_base + 8u * (2 * p.stages + 1 + team * p.aux_depth + slot); };
-  auto aux_empty = [&](int team, int slot) { return bar_base + 8u * (2 * p.stages + 1 + (2 + team) * p.aux_depth + slot); };
+  const FpropSmem L = fprop_smem(p, pingpong, smem_aligned(smem_raw));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -292,13 +292,10 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int s = 0; s < p.stages; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), pingpong ? kConsumerWarps / 2 : kConsumerWarps);   // ping-pong: one warpgroup per stage
-    }
-    for (int a = 0; a < 2; ++a)
-      for (int sl = 0; sl < p.aux_depth; ++sl) { mbar_init(aux_full(a, sl), 1); mbar_init(aux_empty(a, sl), 1); }
-    mbar_init(bres_bar, 1);
+    L.ops.init(pingpong ? kConsumerWarps / 2 : kConsumerWarps);   // ping-pong: one warpgroup per stage
+    L.bres_ready.init(1);
+    L.aux_ring(0).init(1);
+    L.aux_ring(1).init(1);
     fence_barrier_init();
     if (p.use_tma) tma_prefetch_desc(&tmY);
   }
@@ -308,10 +305,10 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     reg_alloc<kConsumerRegs>();
     const int wg = (threadIdx.x - 128) >> 7;
     if constexpr (pingpong) {
-      if (p.BN == 64) fprop_pp_consumer<F, 64>(p, &tmY, smem_base, stage_bytes, bres_base, b_bytes, bar_base, epi_stage_base, aux_stage_base, wg);
-      else fprop_pp_consumer<F, 128>(p, &tmY, smem_base, stage_bytes, bres_base, b_bytes, bar_base, epi_stage_base, aux_stage_base, wg);
+      if (p.BN == 64) fprop_pp_consumer<F, 64>(p, &tmY, L, wg);
+      else fprop_pp_consumer<F, 128>(p, &tmY, L, wg);
     } else {
-      fprop_staged_consumer<F>(p, &tmY, smem_base, stage_bytes, bres_base, b_bytes, bar_base, epi_stage_base, aux_stage_base, acc_base, wg);
+      fprop_staged_consumer<F>(p, &tmY, L, wg);
     }
     return;
   }
@@ -321,10 +318,10 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // ------------------------------------------------------------- TMA producer: one operand ring in tile order
       uint32_t it = 0;
       if (p.b_resident) {       // tiles_n == 1: the whole (small) filter is fetched once per CTA instead of once per tile
-        mbar_arrive_expect_tx(bres_bar, (uint32_t)(p.taps * p.kblocks) * b_bytes);
+        L.bres_ready.acquire(0, (uint32_t)(p.taps * p.kblocks) * L.b_bytes);
         for (int tap = 0; tap < p.taps; ++tap)
           for (int kb = 0; kb < p.kblocks; ++kb)
-            tma_load_3d(bres_base + (uint32_t)(tap * p.kblocks + kb) * b_bytes, &tmB, bres_bar, kb * kBlockK, tap, 0);
+            tma_load_3d(L.bres + (uint32_t)(tap * p.kblocks + kb) * L.b_bytes, &tmB, L.bres_ready.full(0), kb * kBlockK, tap, 0);
       }
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         const FpropTile tc = fprop_tile(p, tile);
@@ -332,20 +329,17 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int tap = 0; tap < p.taps; ++tap) {
           const int dh = tap / p.KW - p.pad_h, dw = tap % p.KW - p.pad_w;
           for (int kb = 0; kb < p.kblocks; ++kb, ++it) {
-            const int s = it % p.stages;
-            const uint32_t ph = (it / p.stages) & 1;
-            mbar_wait(empty_bar(s), ph ^ 1);
-            mbar_arrive_expect_tx(full_bar(s), stage_bytes);
-            const uint32_t sa = smem_base + s * stage_bytes;
-            tma_load_4d(sa, &tmA, full_bar(s), kb * kBlockK, w0 + dw, h0 + dh, b0);
+            const int s = L.ops.acquire(it, L.stage_bytes);
+            const uint32_t sa = L.ring + s * L.stage_bytes, full = L.ops.full(s);
+            tma_load_4d(sa, &tmA, full, kb * kBlockK, w0 + dw, h0 + dh, b0);
             if (p.b_resident) {
             } else if (p.w_mode == 0) {
-              tma_load_3d(sa + kABytes, &tmB, full_bar(s), kb * kBlockK, tap, n0);
+              tma_load_3d(sa + kABytes, &tmB, full, kb * kBlockK, tap, n0);
             } else if (p.w_mode == 1) {
-              tma_load_3d(sa + kABytes, &tmB, full_bar(s), kb * kBlockK, b0, n0);
+              tma_load_3d(sa + kABytes, &tmB, full, kb * kBlockK, b0, n0);
             } else {
               for (int j = 0; j < p.BN / 64; ++j)
-                tma_load_3d(sa + kABytes + j * 8192, &tmB, full_bar(s), n0 + j * 64, kb * kBlockK, b0);
+                tma_load_3d(sa + kABytes + j * 8192, &tmB, full, n0 + j * 64, kb * kBlockK, b0);
             }
           }
         }
@@ -366,10 +360,9 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const int nbase = tc.nt * p.BN + cc * 64;
           if (nbase >= p.e.Cout) break;
           const int team = pingpong ? (i & 1) : (cc & 1);
-          const uint32_t slot = cnt[team] % (uint32_t)p.aux_depth;
-          mbar_wait(aux_empty(team, slot), ((cnt[team] / (uint32_t)p.aux_depth) & 1u) ^ 1u);
-          mbar_arrive_expect_tx(aux_full(team, slot), bytes);
-          tma_load_4d(aux_stage_base + (uint32_t)(team * p.aux_depth + slot) * kEpiStageBytes, &tmAux, aux_full(team, slot), nbase, c1, c2, c3);
+          const MbarRing ring = L.aux_ring(team);
+          const int slot = ring.acquire(cnt[team], bytes);
+          tma_load_4d(L.aux + (uint32_t)(team * p.aux_depth + slot) * kEpiStageBytes, &tmAux, ring.full(slot), nbase, c1, c2, c3);
           ++cnt[team];
         }
       }
@@ -393,6 +386,24 @@ struct WgradArgs {
   float* dbias;                              // optional: sum over pixels of dy (bias gradient), from a constant-ones B operand
 };
 
+// Shared memory of conv_wgrad_kernel: addresses from base, or offsets from the 1024-aligned base when base = 0.
+struct WgradSmem {
+  uint32_t ones;                  // bf16 1.0 slab (dbias)
+  uint32_t ring;                  // operand ring: stages x (two 64-channel dY boxes -> M = 128, BN / 64 X boxes)
+  uint32_t stage_bytes;
+  MbarRing ops;
+  uint32_t total;
+};
+__host__ __device__ inline WgradSmem wgrad_smem(const WgradArgs& p, uint32_t base = 0) {
+  WgradSmem L;
+  L.stage_bytes = 2 * kABytes + (uint32_t)(p.BN / 64) * kABytes;
+  L.ones = base;
+  L.ring = L.ones + (p.dbias ? kOnesSlabBytes : 0u);
+  L.ops = {L.ring + (uint32_t)p.stages * L.stage_bytes, p.stages};
+  L.total = L.ops.end() - base;
+  return L;
+}
+
 // work item -> (m tile, n tile, tap, split); n fastest so neighbouring CTAs share the dY tiles in L2
 __device__ __forceinline__ void wgrad_decode(const WgradArgs& p, int item, int& mt, int& nt, int& tap, int& grp, int& pt_begin,
                                              int& pt_end) {
@@ -410,8 +421,7 @@ __device__ __forceinline__ void wgrad_decode(const WgradArgs& p, int item, int& 
 // One wgrad work item for this consumer warpgroup (output channels mt*128 + 64 wg ..): MMAs over the item's pixel tiles, then
 // fp32 red.adds straight from the accumulator registers.
 template <int BN>
-__device__ __forceinline__ void wgrad_item(const WgradArgs& p, int item, uint32_t smem_base, uint32_t stage_bytes, uint32_t bar_base,
-                                           uint32_t ones_base, uint32_t& it, int wg) {
+__device__ __forceinline__ void wgrad_item(const WgradArgs& p, const WgradSmem& L, int item, uint32_t& it, int wg) {
   int mt, nt, tap, grp, pb, pe;
   wgrad_decode(p, item, mt, nt, tap, grp, pb, pe);
   const uint32_t lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
@@ -423,13 +433,11 @@ __device__ __forceinline__ void wgrad_item(const WgradArgs& p, int item, uint32_
   for (int i = 0; i < 4; ++i) bacc[i] = 0.f;
   // bias gradient: the (first input-channel tile, first tap) items also multiply dY^T by a block of ones (K-major, N = 8)
   const bool with_bias = p.dbias != nullptr && nt == 0 && tap == 0;
-  const uint64_t ones_desc = make_sdesc_sw128(ones_base, 16, 1024);
+  const uint64_t ones_desc = make_sdesc_sw128(L.ones, 16, 1024);
   int prev = -1;
   for (int pt = pb; pt < pe; ++pt, ++it) {
-    const int s = it % p.stages;
-    const uint32_t ph = (it / p.stages) & 1;
-    mbar_wait(bar_base + 8u * s, ph);
-    const uint32_t sa = smem_base + s * stage_bytes;
+    const int s = L.ops.wait(it);
+    const uint32_t sa = L.ring + s * L.stage_bytes;
     // MN-major: 64-wide MN atoms are kABytes apart (LBO), 8-row K groups are 1024 B apart (SBO); this warpgroup's M atom = wg
     const uint64_t adesc = make_sdesc_sw128(sa + (uint32_t)wg * kABytes, kABytes, 1024);
     const uint64_t bdesc = make_sdesc_sw128(sa + a_bytes, kABytes, 1024);
@@ -442,14 +450,12 @@ __device__ __forceinline__ void wgrad_item(const WgradArgs& p, int item, uint32_
       for (int kk = 0; kk < kTileM / 16; ++kk) Wgmma<8>::template mma<1, 0>(bacc, adesc + 128 * kk, ones_desc, 1u);
     }
     wgmma_commit();
-    wgmma_wait<1>();
-    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev)); }
-    prev = s;
+    L.ops.release_prev(prev, s);
   }
   wgmma_wait<0>();
   acc_fence(acc);
   acc_fence(bacc);
-  if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_base + 8u * (p.stages + prev)); }
+  if (prev >= 0) L.ops.release(prev);
   if (pe <= pb) return;
   const int co0 = mt * 128 + wg * 64 + (int)(16u * w + (lane >> 2));
   const int ci0 = nt * BN + 2 * (int)(lane & 3);
@@ -472,30 +478,16 @@ __device__ __forceinline__ void wgrad_item(const WgradArgs& p, int item, uint32_
 __global__ void __launch_bounds__(kWgradThreads, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, const WgradArgs p) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t ones_base = (smem_u32(smem_raw) + 1023u) & ~1023u;          // bf16 1.0 slab when dbias
-  const uint32_t smem_base = ones_base + (p.dbias ? 1024u : 0u);
-  const uint32_t a_bytes = 2 * kABytes;                       // two 64-channel boxes -> M = 128
-  const uint32_t b_bytes = (uint32_t)(p.BN / 64) * kABytes;   // BN/64 boxes
-  const uint32_t stage_bytes = a_bytes + b_bytes;
-  const uint32_t bar_base = smem_base + (uint32_t)p.stages * stage_bytes;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
+  const WgradSmem L = wgrad_smem(p, smem_aligned(smem_raw));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (p.dbias) {
-    for (uint32_t i = threadIdx.x; i < 1024u / 16u; i += kWgradThreads)
-      st_shared_v4(ones_base + i * 16u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u);
-    fence_proxy_async_smem();                 // generic-proxy writes -> visible to the tensor core's operand reads
-  }
+  if (p.dbias) fill_ones_slab(L.ones, kWgradThreads);
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmDY);
     tma_prefetch_desc(&tmX);
-    for (int s = 0; s < p.stages; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), kConsumerWarps);
-    }
+    L.ops.init(kConsumerWarps);
     fence_barrier_init();
   }
   __syncthreads();
@@ -513,15 +505,12 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
           const int ht = t % p.tiles_h; t /= p.tiles_h;
           const int bt = t;
           const int w0 = wt * p.tw, h0 = ht * p.th, b0 = bt * p.nb;
-          const int s = it % p.stages;
-          const uint32_t ph = (it / p.stages) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
-          mbar_arrive_expect_tx(full_bar(s), stage_bytes);
-          const uint32_t sa = smem_base + s * stage_bytes;
-          tma_load_4d(sa, &tmDY, full_bar(s), mt * 128, w0, h0, b0);
-          tma_load_4d(sa + kABytes, &tmDY, full_bar(s), mt * 128 + 64, w0, h0, b0);
+          const int s = L.ops.acquire(it, L.stage_bytes);
+          const uint32_t sa = L.ring + s * L.stage_bytes, full = L.ops.full(s);
+          tma_load_4d(sa, &tmDY, full, mt * 128, w0, h0, b0);
+          tma_load_4d(sa + kABytes, &tmDY, full, mt * 128 + 64, w0, h0, b0);
           for (int j = 0; j < p.BN / 64; ++j)
-            tma_load_4d(sa + a_bytes + j * kABytes, &tmX, full_bar(s), nt * p.BN + j * 64, w0 + dw, h0 + dh, b0);
+            tma_load_4d(sa + 2 * kABytes + j * kABytes, &tmX, full, nt * p.BN + j * 64, w0 + dw, h0 + dh, b0);
         }
       }
     }
@@ -529,8 +518,8 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
     const int wg = (threadIdx.x - 128) >> 7;
     uint32_t it = 0;
     for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-      if (p.BN == 64) wgrad_item<64>(p, item, smem_base, stage_bytes, bar_base, ones_base, it, wg);
-      else wgrad_item<128>(p, item, smem_base, stage_bytes, bar_base, ones_base, it, wg);
+      if (p.BN == 64) wgrad_item<64>(p, L, item, it, wg);
+      else wgrad_item<128>(p, L, item, it, wg);
     }
   }
 }
@@ -680,24 +669,21 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   // ping-pong variants: no fp32 accumulator staging; 8 KiB half-tile staging tiles per warpgroup.  Staged variants: fp32 rows
   // of the whole tile plus 16 KiB staging tiles per epilogue team.
   const bool pingpong = fprop_is_pingpong(f);
-  const int epi_tile_kb = pingpong ? (int)(kFragStageBytes / 1024) : (int)(kEpiStageBytes / 1024);
-  const int acc_kb = pingpong ? 0 : (int)(kTileM * acc_row_bytes(BN) / 1024);
   // short-K layers (one or two K blocks per tile) are store bound: their (small) filter stays resident in shared memory and the
   // space of the B halves of the ring buys more staging tiles per epilogue team = more store bytes in flight
   const uint32_t b_tile = (uint32_t)BN * kBlockK * 2;
   const int kt = p.taps * p.kblocks;
   p.b_resident = (d->w_mode == 0 && p.tiles_n == 1 && kt <= 2 && kt * b_tile <= 64u * 1024u) ? 1 : 0;
-  const uint32_t stage_bytes = kABytes + (p.b_resident ? 0u : b_tile);
   p.epi_nbuf = !p.use_tma ? 1 : pingpong ? (kt <= 2 ? 4 : 2) : (kt <= 2 ? 2 : 1);
   p.aux_depth = p.aux_kind ? 2 : 1;
-  auto ring_kb = [&](int nbuf) {
-    return 216 - acc_kb - (p.use_tma ? 2 * epi_tile_kb * nbuf : 0) - (p.aux_kind ? 32 * p.aux_depth : 0) -
-           (p.b_resident ? (int)(kt * b_tile / 1024) : 0);
-  };
+  p.stages = 0;
+  // room for the operand ring: 216 KiB less the layout in front of it
+  auto ring_room = [&] { return 216 * 1024 - (int)fprop_smem(p, pingpong).ring; };
+  const int stage_bytes = (int)fprop_smem(p, pingpong).stage_bytes;
   // keep >= 3 operand ring stages: give back aux depth first, then staging tiles
-  while (p.aux_kind && p.aux_depth > 1 && ring_kb(p.epi_nbuf) * 1024 < (int)(3 * stage_bytes)) --p.aux_depth;
-  while (p.epi_nbuf > 1 && ring_kb(p.epi_nbuf) * 1024 < (int)(3 * stage_bytes)) --p.epi_nbuf;
-  int stages = ring_kb(p.epi_nbuf) * 1024 / (int)stage_bytes;
+  while (p.aux_kind && p.aux_depth > 1 && ring_room() < 3 * stage_bytes) --p.aux_depth;
+  while (p.epi_nbuf > 1 && ring_room() < 3 * stage_bytes) --p.epi_nbuf;
+  int stages = ring_room() / stage_bytes;
   if (stages > 8) stages = 8;
   if (stages < 2) stages = 2;
   p.stages = stages;
@@ -738,9 +724,7 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
     rc = make_act_tmap(&tmAux, ap, d->B, half ? d->H / 2 : d->H, half ? d->W / 2 : d->W, d->Cout, acs, p.aux_tw, p.aux_th, p.nb);
     if (rc) return rc;
   }
-  const size_t smem = (size_t)stages * stage_bytes + (p.use_tma ? 2 * p.epi_nbuf * epi_tile_kb * 1024 : 0) +
-                      (p.aux_kind ? 2 * p.aux_depth * kEpiStageBytes : 0) + (p.b_resident ? (size_t)kt * b_tile : 0) +
-                      (pingpong ? 0 : (size_t)kTileM * acc_row_bytes(BN)) + 1024 + 8 * (2 * stages + 1 + 4 * 3);
+  const size_t smem = smem_request(fprop_smem(p, pingpong).total);
   SGB_REQUIRE(smem <= 227u * 1024u);
   int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
   return FpropCompiled::launch(f, [&](auto F) {
@@ -807,12 +791,12 @@ extern "C" int sgb_conv_wgrad(const sgb_wgrad_desc* d, sgb_stream_t stream_) {
     p.splits = (p.tiles_per_group + p.tiles_per_split - 1) / p.tiles_per_split;
   }
   p.num_items = base_items * p.splits;
-  const uint32_t stage_bytes = 2 * kABytes + (p.BN / 64) * kABytes;
-  int stages = (int)((216 * 1024) / stage_bytes);
-  if (stages > 6) stages = 6;
-  p.stages = stages;
   p.dw = d->dw;
   p.dbias = d->dbias;
+  p.stages = 0;
+  int stages = (int)((216 * 1024) / wgrad_smem(p).stage_bytes);
+  if (stages > 6) stages = 6;
+  p.stages = stages;
   if (d->dbias && !d->accumulate) SGB_CUDA(cudaMemsetAsync(d->dbias, 0, sizeof(float) * (size_t)d->Cout, stream));
 
   if (!d->accumulate)
@@ -824,7 +808,7 @@ extern "C" int sgb_conv_wgrad(const sgb_wgrad_desc* d, sgb_stream_t stream_) {
   rc = make_act_tmap(&tmX, d->x, d->B, d->H, d->W, d->Cin, d->x_cstride, p.tw, p.th, p.nb);
   if (rc) return rc;
 
-  const size_t smem = (size_t)stages * stage_bytes + (d->dbias ? 1024 : 0) + 1024 + 8 * (2 * stages);
+  const size_t smem = smem_request(wgrad_smem(p).total);
   int grid = p.num_items < sm_count() ? p.num_items : sm_count();
   return launch_kernel<conv_wgrad_kernel>(grid, kWgradThreads, smem, stream, tmDY, tmX, p);
 }

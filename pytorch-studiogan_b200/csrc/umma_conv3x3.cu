@@ -23,6 +23,7 @@ namespace sgb {
 static constexpr int kRowPix = 130;
 static constexpr int kRowLoadBytes = kRowPix * 128;   // 16640
 static constexpr int kRowBufBytes = 17 * 1024;        // 17408, keeps every row buffer 1024-byte aligned
+static constexpr uint32_t kRowStageBytes = 4 * kRowBufBytes;   // one halo stage: input rows h0 - 1 .. h0 + 2
 static constexpr int kRowsConsumers = 256;
 static constexpr int kRowsThreads = 128 + kRowsConsumers;  // warps 0: A producer, 2: B producer, 4..11: MMA + epilogue
 static constexpr uint32_t kRowsAccBar = 3;                 // named barrier of the consumers (1, 2: epilogue teams)
@@ -41,6 +42,29 @@ __host__ __device__ inline uint32_t rows_epi_bytes(const RowsArgs& p) {
   return p.use_tma ? 2u * (uint32_t)p.epi_nbuf * 64u * 128u : 128u * acc_row_bytes(p.BN);
 }
 
+// Shared memory of conv3x3_rows_kernel: addresses from base, or offsets from the 1024-aligned base when base = 0.
+struct RowsSmem {
+  uint32_t epi;                   // rows_epi_bytes
+  uint32_t a;                     // halo ring: a_stages x kRowStageBytes
+  uint32_t b;                     // filter taps: resident [kb][kw][kh], or a ring of b_stages taps
+  uint32_t bar;                   // first barrier = bytes of the tile regions
+  uint32_t b_tile;
+  MbarRing a_ring, b_ring;        // the resident filter is the b ring with one slot, filled once
+  uint32_t total;
+};
+__host__ __device__ inline RowsSmem rows_smem(const RowsArgs& p, uint32_t base = 0) {
+  RowsSmem L;
+  L.b_tile = (uint32_t)p.BN * 128u;
+  L.epi = base;
+  L.a = L.epi + rows_epi_bytes(p);
+  L.b = L.a + (uint32_t)p.a_stages * kRowStageBytes;
+  L.bar = L.b + (p.resident ? 9u * p.kblocks : (uint32_t)p.b_stages) * L.b_tile;
+  L.a_ring = {L.bar, p.a_stages};
+  L.b_ring = {L.a_ring.end(), p.b_stages};
+  L.total = L.b_ring.end() - base;
+  return L;
+}
+
 // Tile index -> (channel tile, 128-pixel segment, row pair, image), channel tiles fastest.
 struct RowsTile { int nt, ws, hp, b; };
 __device__ __forceinline__ RowsTile rows_tile(const RowsArgs& p, int t) {
@@ -54,33 +78,25 @@ __device__ __forceinline__ RowsTile rows_tile(const RowsArgs& p, int t) {
 
 // One work item of a consumer warpgroup: both output rows' MMAs over every K block, accumulators for rows 0 / 1 in acc[0 / 1].
 template <int BN>
-__device__ __forceinline__ void rows_mma_tile(const RowsArgs& p, float (&acc)[2][BN / 2], uint32_t a_base, uint32_t a_stage_bytes,
-                                              uint32_t b_base, uint32_t b_tile_bytes, uint32_t bar_base, int nb, uint32_t& ita,
+__device__ __forceinline__ void rows_mma_tile(const RowsArgs& p, const RowsSmem& L, float (&acc)[2][BN / 2], uint32_t& ita,
                                               uint32_t& itb, int wg) {
-  const uint32_t lane = threadIdx.x & 31;
-  auto a_full = [&](int s) { return bar_base + 8u * s; };
-  auto a_empty = [&](int s) { return bar_base + 8u * (p.a_stages + s); };
-  auto b_full = [&](int s) { return bar_base + 8u * (2 * p.a_stages + s); };
-  auto b_empty = [&](int s) { return bar_base + 8u * (2 * p.a_stages + nb + s); };
 #pragma unroll
   for (int j = 0; j < 2; ++j)
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[j][i] = 0.f;
   for (int kb = 0; kb < p.kblocks; ++kb, ++ita) {
-    const int sa_i = ita % p.a_stages;
-    mbar_wait(a_full(sa_i), (ita / p.a_stages) & 1);
-    const uint32_t sa = a_base + sa_i * a_stage_bytes + (uint32_t)wg * 8192u;   // this warpgroup's 64 pixels
+    const int sa_i = L.a_ring.wait(ita);
+    const uint32_t sa = L.a + sa_i * kRowStageBytes + (uint32_t)wg * 8192u;   // this warpgroup's 64 pixels
     int bprev = -1;                              // filter-ring slot of the previous tap, released once its MMAs retire
     for (int tap = 0; tap < 9; ++tap) {
       const int kh = tap / 3, kw = tap % 3;
       uint32_t sb;
       int bslot = 0;
       if (p.resident) {
-        sb = b_base + ((kb * 3 + kw) * 3 + kh) * b_tile_bytes;     // resident order [kb][kw][kh]
+        sb = L.b + ((kb * 3 + kw) * 3 + kh) * L.b_tile;     // resident order [kb][kw][kh]
       } else {
-        bslot = itb % p.b_stages;
-        mbar_wait(b_full(bslot), (itb / p.b_stages) & 1);
-        sb = b_base + bslot * b_tile_bytes;
+        bslot = L.b_ring.wait(itb);
+        sb = L.b + bslot * L.b_tile;
       }
       const uint64_t bdesc = make_sdesc_sw128(sb, 16, 1024);
       wgmma_fence();
@@ -92,17 +108,13 @@ __device__ __forceinline__ void rows_mma_tile(const RowsArgs& p, float (&acc)[2]
       }
       wgmma_commit();
       if (!p.resident) {
-        wgmma_wait<1>();
-        __syncwarp();
-        if (bprev >= 0 && lane == 0) mbar_arrive(b_empty(bprev));
-        bprev = bslot;
+        L.b_ring.release_prev(bprev, bslot);
         ++itb;
       }
     }
     wgmma_wait<0>();
-    __syncwarp();
-    if (bprev >= 0 && lane == 0) mbar_arrive(b_empty(bprev));
-    if (lane == 0) mbar_arrive(a_empty(sa_i));
+    if (bprev >= 0) L.b_ring.release(bprev);
+    L.a_ring.release(sa_i);
   }
   acc_fence(acc[0]);
   acc_fence(acc[1]);
@@ -117,32 +129,31 @@ __device__ __forceinline__ void rows_stage(const float (&acc)[BN / 2], uint32_t 
 }
 
 template <int F, int BN>
-__device__ __forceinline__ void rows_consumer(const RowsArgs& p, const CUtensorMap* tmY, uint32_t epi_base, uint32_t a_base,
-                                              uint32_t a_stage_bytes, uint32_t b_base, uint32_t b_tile_bytes, uint32_t bar_base, int nb) {
+__device__ __forceinline__ void rows_consumer(const RowsArgs& p, const CUtensorMap* tmY, const RowsSmem& L) {
   const int ct = threadIdx.x - 128;
   const int wg = ct >> 7;
   const int q = (ct >> 5) & 3;
   const int lane = threadIdx.x & 31;
   const float alpha = epi_alpha(p.e);
   uint32_t ita = 0, itb = 0;
-  if (p.resident) mbar_wait(bar_base + 8u * (2 * p.a_stages), 0);
+  if (p.resident) L.b_ring.wait(0);
   if constexpr (F < 0 || BN < 64) {
     if (!p.use_tma) {
       // staged-row epilogue (fp32 output, N < 64, unaligned strides): both rows' accumulators go through shared memory and
       // warpgroup 1 runs epilogue_row, one thread per pixel
       const int row = q * 32 + lane;
       const bool vec_ok = epi_vec_ok(p.e);
-      const uint32_t t_row = epi_base + (uint32_t)row * acc_row_bytes(BN);
+      const uint32_t t_row = L.epi + (uint32_t)row * acc_row_bytes(BN);
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         const RowsTile tc = rows_tile(p, tile);
         const int nt = tc.nt, ws = tc.ws, hp = tc.hp, b = tc.b;
         float acc[2][BN / 2];
-        rows_mma_tile<BN>(p, acc, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb, ita, itb, wg);
+        rows_mma_tile<BN>(p, L, acc, ita, itb, wg);
         const int w = ws * 128 + row;
 #pragma unroll 1
         for (int j = 0; j < 2; ++j) {
-          if (j == 0) rows_stage<BN>(acc[0], epi_base, wg);    // static indices keep both accumulators in registers
-          else rows_stage<BN>(acc[1], epi_base, wg);
+          if (j == 0) rows_stage<BN>(acc[0], L.epi, wg);    // static indices keep both accumulators in registers
+          else rows_stage<BN>(acc[1], L.epi, wg);
           const int h = hp * 2 + j;
           const long long pix = ((long long)b * p.H + h) * p.W + w;
           const long long rpix = epi_rpix(p.e, b, h, w, p.H, p.W, pix);
@@ -155,14 +166,14 @@ __device__ __forceinline__ void rows_consumer(const RowsArgs& p, const CUtensorM
   if constexpr (BN >= 64) {
     // fragment epilogue: each warpgroup stores its 64 pixels of both rows from its registers through its own staging tiles
     const bool leader = (ct & 127) == 0;
-    const uint32_t stage = epi_base + (uint32_t)(wg * p.epi_nbuf) * (64u * 128u);
+    const uint32_t stage = L.epi + (uint32_t)(wg * p.epi_nbuf) * (64u * 128u);
     const uint32_t r0 = 16u * (uint32_t)q + ((uint32_t)lane >> 2);
     uint32_t sbuf = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const RowsTile tc = rows_tile(p, tile);
       const int nt = tc.nt, ws = tc.ws, hp = tc.hp, b = tc.b;
       float acc[2][BN / 2];
-      rows_mma_tile<BN>(p, acc, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb, ita, itb, wg);
+      rows_mma_tile<BN>(p, L, acc, ita, itb, wg);
       const int w0 = ws * 128 + wg * 64;
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
@@ -186,19 +197,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1)
 conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmY, const RowsArgs p) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t epi_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // bf16 staging tiles, or fp32 accumulator rows (!use_tma)
-  const uint32_t smem_base = epi_base + rows_epi_bytes(p);              // 1024-aligned
-  const uint32_t a_stage_bytes = 4 * kRowBufBytes;
-  const uint32_t b_tile_bytes = (uint32_t)p.BN * 128u;
-  const uint32_t a_base = smem_base;
-  const uint32_t b_base = a_base + (uint32_t)p.a_stages * a_stage_bytes;
-  const uint32_t b_total = p.resident ? 9u * p.kblocks * b_tile_bytes : (uint32_t)p.b_stages * b_tile_bytes;
-  const uint32_t bar_base = b_base + b_total;
-  const int nb = p.resident ? 1 : p.b_stages;
-  auto a_full = [&](int s) { return bar_base + 8u * s; };
-  auto a_empty = [&](int s) { return bar_base + 8u * (p.a_stages + s); };
-  auto b_full = [&](int s) { return bar_base + 8u * (2 * p.a_stages + s); };
-  auto b_empty = [&](int s) { return bar_base + 8u * (2 * p.a_stages + nb + s); };
+  const RowsSmem L = rows_smem(p, smem_aligned(smem_raw));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -206,8 +205,8 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int s = 0; s < p.a_stages; ++s) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), kRowsConsumers / 32); }
-    for (int s = 0; s < nb; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), kRowsConsumers / 32); }
+    L.a_ring.init(kRowsConsumers / 32);
+    L.b_ring.init(kRowsConsumers / 32);
     fence_barrier_init();
   }
   __syncthreads();
@@ -215,10 +214,10 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (warp >= 4) {
     reg_alloc<kConsumerRegs>();
     switch (p.BN) {
-      case 16: rows_consumer<F, 16>(p, &tmY, epi_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
-      case 32: rows_consumer<F, 32>(p, &tmY, epi_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
-      case 64: rows_consumer<F, 64>(p, &tmY, epi_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
-      default: rows_consumer<F, 128>(p, &tmY, epi_base, a_base, a_stage_bytes, b_base, b_tile_bytes, bar_base, nb); break;
+      case 16: rows_consumer<F, 16>(p, &tmY, L); break;
+      case 32: rows_consumer<F, 32>(p, &tmY, L); break;
+      case 64: rows_consumer<F, 64>(p, &tmY, L); break;
+      default: rows_consumer<F, 128>(p, &tmY, L); break;
     }
     return;
   }
@@ -231,11 +230,9 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         const RowsTile tc = rows_tile(p, tile);
         const int w0 = tc.ws * 128, h0 = tc.hp * 2, b = tc.b;
         for (int kb = 0; kb < p.kblocks; ++kb, ++it) {
-          const int s = it % p.a_stages;
-          mbar_wait(a_empty(s), ((it / p.a_stages) & 1) ^ 1);
-          mbar_arrive_expect_tx(a_full(s), 4 * kRowLoadBytes);
-          const uint32_t sa = a_base + s * a_stage_bytes;
-          for (int r = 0; r < 4; ++r) tma_load_4d(sa + r * kRowBufBytes, &tmA, a_full(s), kb * 64, w0 - 1, h0 - 1 + r, b);
+          const int s = L.a_ring.acquire(it, 4 * kRowLoadBytes);
+          const uint32_t sa = L.a + s * kRowStageBytes;
+          for (int r = 0; r < 4; ++r) tma_load_4d(sa + r * kRowBufBytes, &tmA, L.a_ring.full(s), kb * 64, w0 - 1, h0 - 1 + r, b);
         }
       }
     }
@@ -243,20 +240,18 @@ conv3x3_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     if (lane == 0) {
       // ------------------------------------------------------------- B producer: filter taps (resident or ring)
       if (p.resident) {
-        mbar_arrive_expect_tx(b_full(0), 9u * p.kblocks * b_tile_bytes);
+        L.b_ring.acquire(0, 9u * p.kblocks * L.b_tile);
         for (int tap = 0; tap < 9; ++tap)
           for (int kb = 0; kb < p.kblocks; ++kb)
-            tma_load_3d(b_base + ((kb * 3 + tap % 3) * 3 + tap / 3) * b_tile_bytes, &tmB, b_full(0), kb * 64, tap, 0);
+            tma_load_3d(L.b + ((kb * 3 + tap % 3) * 3 + tap / 3) * L.b_tile, &tmB, L.b_ring.full(0), kb * 64, tap, 0);
       } else {
         uint32_t it = 0;
         for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
           const int nt = rows_tile(p, tile).nt;
           for (int kb = 0; kb < p.kblocks; ++kb)
             for (int tap = 0; tap < 9; ++tap, ++it) {
-              const int s = it % p.b_stages;
-              mbar_wait(b_empty(s), ((it / p.b_stages) & 1) ^ 1);
-              mbar_arrive_expect_tx(b_full(s), b_tile_bytes);
-              tma_load_3d(b_base + s * b_tile_bytes, &tmB, b_full(s), kb * 64, tap, nt * p.BN);
+              const int s = L.b_ring.acquire(it, L.b_tile);
+              tma_load_3d(L.b + s * L.b_tile, &tmB, L.b_ring.full(s), kb * 64, tap, nt * p.BN);
             }
         }
       }
@@ -290,26 +285,25 @@ int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream) {
   p.segs = d->W / 128;
   p.hpairs = d->H / 2;
   p.num_tiles = p.tiles_n * p.segs * p.hpairs * d->B;
-  const uint32_t b_tile = p.BN * 128u;
   const uint32_t budget = 227u * 1024u - 2048u;
-  const uint32_t a_stage = 4 * kRowBufBytes;
-  const uint32_t resident_bytes = 9u * p.kblocks * b_tile;
   p.use_tma = epi_tma_ok(d, p.BN) ? 1 : 0;
+  // tile bytes of the layout with a halo stages and b filter stages (the whole filter when resident)
+  auto tiles = [&](int a, int b) { p.a_stages = a; p.b_stages = b; return rows_smem(p).bar; };
   // two staging tiles per warpgroup (a chunk's store overlaps the next chunk's packing), one where that would cost the
   // resident filter its second halo stage (C = 64: 72 KiB taps + 2 x 68 KiB halo + 16 KiB staging)
   p.epi_nbuf = 2;
-  p.resident = (p.tiles_n == 1 && resident_bytes + a_stage + rows_epi_bytes(p) <= budget) ? 1 : 0;
-  if (p.resident && p.use_tma && resident_bytes + 2 * a_stage + rows_epi_bytes(p) > budget) p.epi_nbuf = 1;
-  const uint32_t fixed = rows_epi_bytes(p);
+  p.resident = 1;
+  if (p.tiles_n != 1 || tiles(1, 1) > budget) p.resident = 0;
+  if (p.resident && p.use_tma && tiles(2, 1) > budget) p.epi_nbuf = 1;
   if (p.resident) {
-    p.a_stages = (int)((budget - resident_bytes - fixed) / a_stage);
-    if (p.a_stages > 3) p.a_stages = 3;
+    const int a_stages = (int)((budget - tiles(0, 1)) / kRowStageBytes);
+    p.a_stages = a_stages > 3 ? 3 : a_stages;
     p.b_stages = 1;
   } else {
-    p.a_stages = 2;
-    if (2 * a_stage + fixed + 2 * b_tile > budget) p.a_stages = 1;
-    p.b_stages = (int)((budget - p.a_stages * a_stage - fixed) / b_tile);
-    if (p.b_stages > 6) p.b_stages = 6;
+    const int a_stages = tiles(2, 2) > budget ? 1 : 2;
+    const int b_stages = (int)((budget - tiles(a_stages, 0)) / rows_smem(p).b_tile);
+    p.a_stages = a_stages;
+    p.b_stages = b_stages > 6 ? 6 : b_stages;
     if (p.b_stages < 2) return SGB_ERR_UNSUPPORTED;
   }
   fill_epi(p.e, d);
@@ -329,9 +323,7 @@ int launch_conv3x3_rows(const sgb_conv_desc* d, cudaStream_t stream) {
     rc = make_act_tmap(&tmY, d->y, d->B, d->H, d->W, d->Cout, d->y_cstride, 64, 1, 1);   // one warpgroup's 64 pixels
     if (rc) return rc;
   }
-  const int nb = p.resident ? 1 : p.b_stages;
-  const size_t smem = (size_t)p.a_stages * a_stage + (p.resident ? resident_bytes : p.b_stages * b_tile) + fixed + 1024 +
-                      8 * (2 * p.a_stages + 2 * nb);
+  const size_t smem = smem_request(rows_smem(p).total);
   SGB_REQUIRE(smem <= 227u * 1024u);
   const int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
   const int f = p.use_tma ? epi_flags_of(p.e) : -1;

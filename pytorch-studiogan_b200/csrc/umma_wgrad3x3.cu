@@ -34,14 +34,27 @@ struct W3Args {
   float* dbias;                  // optional: sum of dY over all pixels
 };
 
+// Shared memory of wgrad3x3_c64_kernel: addresses from base, or offsets from the 1024-aligned base when base = 0.
+struct W3Smem {
+  uint32_t ring;                  // kW3Stages x (dY tile, X halo)
+  uint32_t ones;                  // bf16 1.0 slab
+  MbarRing ops;
+  uint32_t total;
+};
+__host__ __device__ inline W3Smem w3_smem(uint32_t base = 0) {
+  W3Smem L;
+  L.ring = base;
+  L.ones = L.ring + kW3Stages * kW3Stage;
+  L.ops = {L.ones + kOnesSlabBytes, kW3Stages};
+  L.total = L.ops.end() - base;
+  return L;
+}
+
 // Consumer warpgroup of filter row kh: taps (kh, 0..2) over the CTA's tile range, then the red.add drain.  BIAS: this
 // warpgroup also accumulates dY^T times a constant-ones operand (the bias gradient).
 template <bool BIAS>
-__device__ __forceinline__ void w3_consumer(const W3Args& p, uint32_t smem_base, uint32_t ones_base, uint32_t bar_base,
-                                            long long t_begin, long long t_end, int kh) {
+__device__ __forceinline__ void w3_consumer(const W3Args& p, const W3Smem& L, long long t_begin, long long t_end, int kh) {
   const int lane = threadIdx.x & 31;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (kW3Stages + s); };
   float acc[3][32], bacc[4];
 #pragma unroll
   for (int k = 0; k < 3; ++k)
@@ -49,14 +62,12 @@ __device__ __forceinline__ void w3_consumer(const W3Args& p, uint32_t smem_base,
     for (int i = 0; i < 32; ++i) acc[k][i] = 0.f;
 #pragma unroll
   for (int i = 0; i < 4; ++i) bacc[i] = 0.f;
-  const uint64_t ones_desc = make_sdesc_sw128(ones_base, 16, 1024);   // K-major N = 8: every element is 1.0
+  const uint64_t ones_desc = make_sdesc_sw128(L.ones, 16, 1024);   // K-major N = 8: every element is 1.0
   uint32_t it = 0;
   int prev = -1;
   for (long long t = t_begin; t < t_end; ++t, ++it) {
-    const int s = it % kW3Stages;
-    const uint32_t ph = (it / kW3Stages) & 1;
-    mbar_wait(full_bar(s), ph);
-    const uint32_t ys = smem_base + s * kW3Stage;
+    const int s = L.ops.wait(it);
+    const uint32_t ys = L.ring + s * kW3Stage;
     const uint32_t xs = ys + kW3DyBytes;
     wgmma_fence();
 #pragma unroll
@@ -75,16 +86,13 @@ __device__ __forceinline__ void w3_consumer(const W3Args& p, uint32_t smem_base,
       }
     }
     wgmma_commit();
-    wgmma_wait<1>();
-    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar(prev)); }
-    prev = s;
+    L.ops.release_prev(prev, s);
   }
   wgmma_wait<0>();
 #pragma unroll
   for (int k = 0; k < 3; ++k) acc_fence(acc[k]);
   acc_fence(bacc);
-  __syncwarp();
-  if (lane == 0) mbar_arrive(empty_bar(prev));
+  L.ops.release(prev);
   // drain: fragment rows = input channels, columns = output channels
   const int w = (threadIdx.x >> 5) & 3;
   const int ci0 = 16 * w + (lane >> 2), co0 = 2 * (lane & 3);
@@ -110,11 +118,7 @@ __device__ __forceinline__ void w3_consumer(const W3Args& p, uint32_t smem_base,
 __global__ void __launch_bounds__(kW3Threads, 1)
 wgrad3x3_c64_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, const W3Args p) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t ones_base = smem_base + kW3Stages * kW3Stage;          // 1 KB of bf16 1.0 (8 rows x 128 B)
-  const uint32_t bar_base = ones_base + 1024u;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (kW3Stages + s); };
+  const W3Smem L = w3_smem(smem_aligned(smem_raw));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -122,17 +126,10 @@ wgrad3x3_c64_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_const
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmDY);
     tma_prefetch_desc(&tmX);
-    for (int s = 0; s < kW3Stages; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), kW3Consumers / 32);
-    }
+    L.ops.init(kW3Consumers / 32);
     fence_barrier_init();
   }
-  if (p.dbias) {
-    for (int i = threadIdx.x; i < 1024 / 4; i += kW3Threads)
-      asm volatile("st.shared.u32 [%0], %1;" ::"r"(ones_base + 4u * i), "r"(0x3F803F80u) : "memory");
-    fence_proxy_async_smem();                     // the MMA reads this region through the async proxy
-  }
+  if (p.dbias) fill_ones_slab(L.ones, kW3Threads);
   __syncthreads();
 
   // contiguous tile range of this CTA
@@ -147,20 +144,17 @@ wgrad3x3_c64_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_const
         const int ht = (int)((t / p.tiles_w) % p.tiles_h);
         const int b = (int)(t / ((long long)p.tiles_w * p.tiles_h));
         const int w0 = wt * kW3Px, h0 = ht * 2;
-        const int s = it % kW3Stages;
-        const uint32_t ph = (it / kW3Stages) & 1;
-        mbar_wait(empty_bar(s), ph ^ 1);
-        mbar_arrive_expect_tx(full_bar(s), kW3DyBytes + kW3XBytes);
-        const uint32_t sa = smem_base + s * kW3Stage;
-        tma_load_4d(sa, &tmDY, full_bar(s), 0, w0, h0, b);
-        tma_load_4d(sa + kW3DyBytes, &tmX, full_bar(s), 0, w0 - 1, h0 - 1, b);   // out-of-range halo = zero padding
+        const int s = L.ops.acquire(it, kW3DyBytes + kW3XBytes);
+        const uint32_t sa = L.ring + s * kW3Stage;
+        tma_load_4d(sa, &tmDY, L.ops.full(s), 0, w0, h0, b);
+        tma_load_4d(sa + kW3DyBytes, &tmX, L.ops.full(s), 0, w0 - 1, h0 - 1, b);   // out-of-range halo = zero padding
       }
     }
   } else if (warp >= 4 && t_end > t_begin) {
     const int kh = (threadIdx.x - 128) >> 7;    // this warpgroup's filter row
     // the bias product is a compile-time property of the consumer body: a branch between the wgmmas would serialise them
-    if (p.dbias != nullptr && kh == 0) w3_consumer<true>(p, smem_base, ones_base, bar_base, t_begin, t_end, kh);
-    else w3_consumer<false>(p, smem_base, ones_base, bar_base, t_begin, t_end, kh);
+    if (p.dbias != nullptr && kh == 0) w3_consumer<true>(p, L, t_begin, t_end, kh);
+    else w3_consumer<false>(p, L, t_begin, t_end, kh);
   }
 }
 
@@ -180,7 +174,7 @@ int launch_wgrad3x3_c64(const sgb_wgrad_desc* d, cudaStream_t stream) {
   CUtensorMap tmDY;
   int rc = make_act_tmap(&tmDY, d->dy, d->B, d->H, d->W, d->Cout, d->dy_cstride, kW3Px, 2, 1);
   if (rc) return rc;
-  const size_t smem = (size_t)kW3Stages * kW3Stage + 1024 + 1024 + 8 * (2 * kW3Stages);
+  const size_t smem = smem_request(w3_smem().total);
   for (int ci0 = 0; ci0 < d->Cin; ci0 += 64) {
     W3Args p;
     p.H = d->H; p.W = d->W; p.Cout = d->Cout;
