@@ -81,7 +81,7 @@ typedef struct sgb_conv_desc {
   /* Row softmax of the attention map (src/utils/ops.py:93-97) inside the GEMM epilogue, 1x1 / w_mode 1 launches with
    * Cout = keys (multiple of 64), bf16 output, no other epilogue operand:
    *   sm_mode 1: statistics pass -- nothing is stored to y; sm_stats[row][part] = (max, sum exp(. - max)) over the columns of one
-   *              (channel tile, epilogue team) pair; parts per row = sgb_conv_softmax_parts(desc)
+   *              output-channel tile (128 channels; 64 when Cout = 64); parts per row = sgb_conv_softmax_parts(desc)
    *   sm_mode 2: y = exp(acc - m_row) / l_row with (m, l) merged from sm_stats (the same GEMM launched a second time)
    *   sm_mode 3: y = sm_p * (acc - sm_delta[row]): softmax backward dS = P * (dP - delta), delta = rowsum(dO * O) */
   int32_t sm_mode;

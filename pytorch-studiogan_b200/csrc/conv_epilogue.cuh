@@ -1,9 +1,10 @@
 // Fused conv epilogue shared by the wgmma conv kernels: accumulator -> alpha, bias, residual (optionally read from a
-// half-resolution tensor = nearest x2 upsample), ReLU, ReLU-mask, post-mask residual -> bf16 / fp32 NHWC store.
+// half-resolution tensor = nearest x2 upsample), ReLU, ReLU-mask, post-mask residual -> bf16 / fp32 NHWC store; or the
+// attention's row softmax (apply / backward) in place of those steps.
 // The questions of a variant are EpiOps<F>; the TMA-store epilogues share the arithmetic epi_pair (one bf16 pair of channels)
 // and only differ in where they load its operands from:
-//   epilogue_tile_tma  : fp32 accumulator rows staged in shared memory, aux tile in shared memory (run-time flags, softmax)
-//   epilogue_frag_chunk: straight from the wgmma accumulator registers
+//   epilogue_tile_tma  : fp32 accumulator rows staged in shared memory, aux tile in shared memory (run-time flags)
+//   epilogue_frag_chunk: straight from the wgmma accumulator registers (every compile-time variant)
 // epilogue_row (direct stores, fp32 outputs, ragged channel tails) keeps 16-wide blocks per question: with run-time flags,
 // per-pair tests of each question are if-converted into selects on every element.
 #pragma once
@@ -26,12 +27,12 @@ struct EpiArgs {
   // mask_bits replaces ``mask`` (1/16 of its bytes); relu_bits is written by a relu epilogue for the consumer's backward.
   const unsigned long long* mask_bits;
   unsigned long long* relu_bits;
-  // Row softmax of the attention map inside the GEMM epilogues (one thread = one query row of the tile):
-  //   sm_mode 1: no output; per row and per (channel tile, team) the partial (max, sum exp) of its columns -> sm_stats
+  // Row softmax of the attention map inside the GEMM epilogues (a query row of a tile is held by the four lanes of a quad):
+  //   sm_mode 1: no output; per row and per channel tile the partial (max, sum exp) of its columns -> sm_stats
   //   sm_mode 2: y = exp(acc - m) / l with (m, l) merged from the row's sm_parts partials
   //   sm_mode 3: y = P * (acc - delta[row]) (softmax backward; P arrives through the aux TMA ring, kind 3)
   int sm_mode, sm_parts;
-  float* sm_stats;            // [rows][sm_parts][2]
+  float* sm_stats;            // [rows][sm_parts = channel tiles][2]
   const float* sm_delta;      // [rows]
 };
 
@@ -82,6 +83,7 @@ template <int F>
 struct EpiOps {
   bool bias, relu, res_pre, res_post, mask, mask_bits, bits_out;
   bool full_c;                                   // no channel-tail tests (F >= 0 only)
+  bool sm_apply, sm_bwd;                         // softmax apply / backward (F >= 0 only)
   __device__ __forceinline__ explicit EpiOps(const EpiArgs& p)
       : bias(F < 0 ? p.bias != nullptr : (F & kEpiBias) != 0),
         relu(F < 0 ? p.relu != 0 : (F & kEpiRelu) != 0),
@@ -90,16 +92,31 @@ struct EpiOps {
         mask(F < 0 ? (p.mask != nullptr || p.mask_bits != nullptr) : (F & kEpiMask) != 0),
         mask_bits(F < 0 ? p.mask_bits != nullptr : (F & kEpiMaskBits) != 0),
         bits_out(F < 0 ? (p.relu != 0 && p.relu_bits != nullptr) : (F & kEpiBitsOut) != 0),
-        full_c(F >= 0 && (F & kEpiFull) != 0) {}
+        full_c(F >= 0 && (F & kEpiFull) != 0),
+        sm_apply(F >= 0 && (F & kEpiSmApply) != 0),
+        sm_bwd(F >= 0 && (F & kEpiSmBwd) != 0) {}
 };
+
+// 2^x on the SFU (ex2.approx: 2^-22 relative error, far below the bf16 rounding of the softmax output); the accurate exp2f
+// costs ~10 instructions per element and made the softmax epilogues issue bound
+__device__ __forceinline__ float fast_ex2(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+static constexpr float kLog2e = 1.4426950408889634f;
 
 // The arithmetic that follows acc * alpha, for two adjacent channels (c, c + 1): + bias, fmaf(residual, rs, .), ReLU, mask,
 // fmaf(post-mask residual, rs, .).  res / msk: the packed bf16 residual / mask pair (low half = channel c); mbits: the pair's
 // two mask bits (bit plane).  pos: bit 0 / 1 set iff the ReLU output of channel c / c + 1 is positive.
+// Softmax variants instead: apply exp(f - m) / l with sm = (-m log2e, 1 / l) of the row; backward P * (f - delta) with
+// sm.x = delta of the row and res = the packed bf16 P pair.
 template <int F>
 __device__ __forceinline__ float2 epi_pair(const EpiOps<F>& op, float f0, float f1, float2 b, uint32_t res, uint32_t msk,
-                                           uint32_t mbits, float rs, uint32_t& pos) {
+                                           uint32_t mbits, float rs, float2 sm, uint32_t& pos) {
   pos = 0u;
+  if (op.sm_apply) { f0 = fast_ex2(fmaf(f0, kLog2e, sm.x)) * sm.y; f1 = fast_ex2(fmaf(f1, kLog2e, sm.x)) * sm.y; }
+  if (op.sm_bwd) { f0 = bf16_bits_lo(res) * (f0 - sm.x); f1 = bf16_bits_hi(res) * (f1 - sm.x); }
   if (op.bias) { f0 += b.x; f1 += b.y; }
   if (op.res_pre) { f0 = fmaf(bf16_bits_lo(res), rs, f0); f1 = fmaf(bf16_bits_hi(res), rs, f1); }
   if (op.relu) {
@@ -284,80 +301,23 @@ __device__ __forceinline__ uint32_t epi_stage_next(uint32_t stage, uint32_t tile
   return cur;
 }
 
-// 2^x on the SFU (ex2.approx: 2^-22 relative error, far below the bf16 rounding of the softmax output); the accurate exp2f
-// costs ~10 instructions per element and made the softmax epilogues issue bound
-__device__ __forceinline__ float fast_ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-// Softmax statistics of one accumulator tile (sm_mode 1): this thread's row, the 64-column chunks of its team; the running
-// (max, sum exp) pair is kept in registers and stored once -- nothing else leaves the SM.
-__device__ __forceinline__ void epilogue_tile_smstats(const EpiArgs& p, uint32_t t_row, int BN, int n0, bool valid, long long pix,
-                                                      float alpha, int team, int part) {
-  float m = -INFINITY, l = 0.f;
-  constexpr float kLog2e = 1.4426950408889634f;
-  for (int cc = team; cc * 64 < BN; cc += 2) {
-    if (n0 + cc * 64 >= p.Cout) break;
-#pragma unroll 1
-    for (int s0 = 0; s0 < 4; s0 += 2) {
-      uint32_t v[2][16];
-      acc_ld16(t_row + 4u * (cc * 64 + s0 * 16), v[0]);
-      acc_ld16(t_row + 4u * (cc * 64 + (s0 + 1) * 16), v[1]);
-      float pm = -INFINITY;
-#pragma unroll
-      for (int q = 0; q < 2; ++q)
-#pragma unroll
-        for (int j = 0; j < 16; ++j) pm = fmaxf(pm, __uint_as_float(v[q][j]) * alpha);
-      const float mn = fmaxf(m, pm);
-      float acc = 0.f;
-      const float a2 = alpha * kLog2e, mn2 = -mn * kLog2e;
-#pragma unroll
-      for (int q = 0; q < 2; ++q)
-#pragma unroll
-        for (int j = 0; j < 16; ++j) acc += fast_ex2(fmaf(__uint_as_float(v[q][j]), a2, mn2));
-      l = l * fast_ex2((m - mn) * kLog2e) + acc;
-      m = mn;
-    }
-  }
-  if (valid) {
-    float2* dst = reinterpret_cast<float2*>(p.sm_stats) + pix * p.sm_parts + part;
-    *dst = make_float2(m, l);
-  }
-}
-
-// Staged epilogue of the run-time general kernel (F = -1) and of the softmax apply / backward variants.
+// Staged epilogue of the run-time general kernel (F = -1).
 // t_row : shared-memory address of this thread's accumulator row (first column of the accumulator).
 // c1..c3: box coordinates (w0, h0, b0) of the tile in the output tensor map; channel coordinate = n0 + chunk * 64.
 // stage : this team's first staging tile (1024-byte aligned), nbuf tiles used round-robin (sbuf = next one).
 // team in {0,1}; row = accumulator row of this thread.  aux: the team's aux ring, or nullptr.
 // A thread converts all four 16-column pieces of its row of the chunk; a team is 4 warps.
-template <int F>
 __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtensorMap* tmY, uint32_t t_row, int BN, int n0,
                                                   int c1, int c2, int c3, bool valid, long long pix, long long rpix, float alpha,
                                                   uint32_t stage, int nbuf, uint32_t& sbuf, int team, int row, bool leader,
                                                   const EpiAux* aux) {
-  static_assert(F == -1 || (F & (kEpiSmApply | kEpiSmBwd)) != 0, "other compile-time variants use epilogue_frag_chunk");
   constexpr int kTeamThreads = 128;
-  constexpr bool sm_apply = F >= 0 && (F & kEpiSmApply) != 0, sm_bwd = F >= 0 && (F & kEpiSmBwd) != 0;
-  constexpr float kLog2e = 1.4426950408889634f;
-  float sm_a = 0.f, sm_b = 1.f;                    // apply: (row max, 1 / row sum); backward: (delta, -)
-  if (sm_apply && valid) {
-    const float2* st = reinterpret_cast<const float2*>(p.sm_stats) + pix * p.sm_parts;
-    float m = -INFINITY;
-    for (int i = 0; i < p.sm_parts; ++i) m = fmaxf(m, __ldcg(&st[i].x));
-    float l = 0.f;
-    for (int i = 0; i < p.sm_parts; ++i) { const float2 t = __ldcg(&st[i]); l += t.y * fast_ex2((t.x - m) * kLog2e); }
-    sm_a = -m * kLog2e; sm_b = 1.f / l;          // exponent offset in base-2 units
-  }
-  if (sm_bwd && valid) sm_a = __ldg(p.sm_delta + pix);
-  const EpiOps<F> op(p);
+  const EpiOps<-1> op(p);
   const long long nw = p.Cout >> 6;
   const float rs = p.res_scale;
   const uint32_t sw = (uint32_t)(row & 7);
-  // 1: residual tile via TMA, 2: mask tile via TMA, 3: the softmax backward's P tile
-  const int aux_kind = F >= 0 ? (sm_bwd ? 3 : 0) : (aux ? aux->kind : 0);
+  // 1: residual tile via TMA, 2: mask tile via TMA
+  const int aux_kind = aux ? aux->kind : 0;
   const uint32_t asw = aux ? (uint32_t)(aux->arow & 7) : 0u;
   for (int cc = team; cc * 64 < BN; cc += 2) {
     const int nbase = n0 + cc * 64;
@@ -371,13 +331,11 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
     const uint32_t srow = stage_cur + (uint32_t)row * 128u;
     named_bar_sync(1 + team, kTeamThreads);
     uint32_t arow_addr = 0u, aslot = 0u;
-    if (aux_kind) {                              // residual / mask / P chunk: one TMA box (fetched ahead by the aux producer warp)
+    if (aux_kind) {                              // residual / mask chunk: one TMA box (fetched ahead by the aux producer warp)
       aslot = aux->ring.wait(*aux->cnt);
       arow_addr = aux->tiles + aslot * kEpiStageBytes + (uint32_t)aux->arow * 128u;
       *aux->cnt += 1u;
     }
-    // compile-time variants handle two 16-column pieces per iteration: both accumulator loads are in flight together
-    constexpr int NP = F >= 0 ? 2 : 1;
     auto piece = [&](const int s, const uint32_t (&v)[16], const uint32_t mb) -> uint32_t {
         const int n = nbase + s * 16;
         float f[16];
@@ -393,18 +351,6 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
                                              : ((op.full_c || 8 * j < nvalid) ? __ldg(reinterpret_cast<const uint4*>(src) + j)
                                                                              : make_uint4(0u, 0u, 0u, 0u));
         };
-        if (sm_apply) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) f[j] = fast_ex2(fmaf(f[j], kLog2e, sm_a)) * sm_b;
-        }
-        if (sm_bwd) {                                // dS = P * (dP - delta); P: this row of the aux tile
-          uint32_t pw[8];
-          load16(3, nullptr, pw);
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            f[2 * k] = bf16_bits_lo(pw[k]) * (f[2 * k] - sm_a); f[2 * k + 1] = bf16_bits_hi(pw[k]) * (f[2 * k + 1] - sm_a);
-          }
-        }
         float b[16] = {};
         uint32_t r[8] = {}, m[8] = {}, w[8];
         if (op.bias && in_c) {
@@ -418,7 +364,8 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
           uint32_t pos;
-          const float2 o = epi_pair(op, f[2 * k], f[2 * k + 1], make_float2(b[2 * k], b[2 * k + 1]), r[k], m[k], mb >> (2 * k), rs, pos);
+          const float2 o = epi_pair(op, f[2 * k], f[2 * k + 1], make_float2(b[2 * k], b[2 * k + 1]), r[k], m[k], mb >> (2 * k), rs,
+                                    make_float2(0.f, 1.f), pos);
           ob |= pos << (2 * k);
           w[k] = pack_bf16x2(o.x, o.y);
         }
@@ -428,17 +375,12 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
         return ob;
     };
 #pragma unroll 1
-    for (int s0 = 0; s0 < 4; s0 += NP) {
-      uint32_t v[NP][16];
-#pragma unroll
-      for (int q = 0; q < NP; ++q) acc_ld16(t_row + 4u * (cc * 64 + (s0 + q) * 16), v[q]);
-#pragma unroll
-      for (int q = 0; q < NP; ++q) {
-        const int s = s0 + q;
-        const uint32_t ob = piece(s, v[q], ((s < 2 ? mlo : mhi) >> (16 * (s & 1))) & 0xFFFFu);
-        if (s < 2) olo |= ob << (16 * (s & 1));
-        else ohi |= ob << (16 * (s & 1));
-      }
+    for (int s = 0; s < 4; ++s) {
+      uint32_t v[16];
+      acc_ld16(t_row + 4u * (cc * 64 + s * 16), v);
+      const uint32_t ob = piece(s, v, ((s < 2 ? mlo : mhi) >> (16 * (s & 1))) & 0xFFFFu);
+      if (s < 2) olo |= ob << (16 * (s & 1));
+      else ohi |= ob << (16 * (s & 1));
     }
     if (op.bits_out && valid) {
       reinterpret_cast<uint2*>(p.relu_bits)[pix * nw + (nbase >> 6)] = make_uint2(olo, ohi);
@@ -464,8 +406,10 @@ __device__ __forceinline__ void epilogue_tile_tma(const EpiArgs& p, const CUtens
 //                clipped by the TMA store; their global loads read pixel 0 and their bit-plane words are not written).
 //   stage      : this warpgroup's first staging tile (1024-aligned), nbuf (1..4) tiles used round-robin (sbuf = next one).
 //   bar        : named barrier of the warpgroup.
-//   aux_tile   : F with kEpiAuxRes / kEpiAuxMask: the chunk's residual / mask box (SWIZZLE_128B, 128-byte rows) filled by the
-//                aux producer; arow = the box row of each of this thread's two rows.  Other variants read global memory.
+//   aux_tile   : F with kEpiAuxRes / kEpiAuxMask / kEpiSmBwd: the chunk's residual / mask / P box (SWIZZLE_128B, 128-byte
+//                rows) filled by the aux producer; arow = the box row of each of this thread's two rows.  Other variants read
+//                global memory.
+//   sm         : softmax apply / backward: epi_pair's row constants of this thread's two rows (sm_row_apply, sm_delta).
 static constexpr uint32_t kFragStageBytes = 64 * 128;
 
 template <int F, int BN>
@@ -473,9 +417,8 @@ __device__ __forceinline__ void epilogue_frag_chunk(const EpiArgs& p, const CUte
                                                     int nbase, int c1, int c2, int c3, const long long (&pix)[2],
                                                     const long long (&rpix)[2], const bool (&valid)[2], float alpha, uint32_t stage,
                                                     int nbuf, uint32_t& sbuf, uint32_t bar, bool leader, uint32_t aux_tile = 0u,
-                                                    const uint32_t (&arow)[2] = {0u, 0u}) {
-  static_assert(F < 0 || (F & (kEpiSmStats | kEpiSmApply | kEpiSmBwd)) == 0, "softmax epilogues are served by epilogue_tile_tma");
-  constexpr int aux_kind = F < 0 ? 0 : ((F & kEpiAuxRes) ? 1 : ((F & kEpiAuxMask) ? 2 : 0));
+                                                    const uint32_t (&arow)[2] = {0u, 0u}, const float2 (&sm)[2] = {}) {
+  constexpr int aux_kind = F < 0 ? 0 : ((F & kEpiAuxRes) ? 1 : ((F & kEpiAuxMask) ? 2 : ((F & kEpiSmBwd) ? 3 : 0)));
   // the ReLU is the last arithmetic of the pair (no mask, no post-mask residual): take the bits from the packed output word --
   // adding 0x7FFF to a post-ReLU bf16 half (+0 or a positive value <= 0x7F80) sets its bit 15 iff it is non-zero, without
   // carrying into its neighbour; fewer instructions than a compare per element, and the bit plane is paid for by write-bound layers
@@ -510,13 +453,13 @@ __device__ __forceinline__ void epilogue_frag_chunk(const EpiArgs& p, const CUte
       // this pair's 4 bytes in the aux box: 16-byte unit jj of row arow sits at jj ^ (arow & 7), conflict-free like the staging
       const uint32_t aaddr = aux_tile + arow[hr] * 128u + ((((uint32_t)jj) ^ (arow[hr] & 7u)) << 4) + 4u * q;
       uint32_t res = 0u, msk = 0u, pos;
-      if ((op.res_pre || op.res_post) && in_c)
-        res = aux_kind == 1 ? ld_shared_b32(aaddr)
-                            : __ldg(reinterpret_cast<const unsigned int*>(p.residual + lrpix[hr] * p.res_cstride + n));
+      if ((op.res_pre || op.res_post || op.sm_bwd) && in_c)
+        res = (aux_kind == 1 || aux_kind == 3) ? ld_shared_b32(aaddr)
+                                               : __ldg(reinterpret_cast<const unsigned int*>(p.residual + lrpix[hr] * p.res_cstride + n));
       if (op.mask && !op.mask_bits && in_c)
         msk = aux_kind == 2 ? ld_shared_b32(aaddr) : __ldg(reinterpret_cast<const unsigned int*>(p.mask + lpix[hr] * p.mask_cstride + n));
       const float2 o = epi_pair(op, acc[4 * j + 2 * hr] * alpha, acc[4 * j + 2 * hr + 1] * alpha, bb, res, msk,
-                                mb[hr][jj >> 2] >> bit, rs, pos);
+                                mb[hr][jj >> 2] >> bit, rs, sm[hr], pos);
       const uint32_t pk = pack_bf16x2(o.x, o.y);
       if (bits_from_packed) {
         const uint32_t t = pk + 0x7FFF7FFFu;
@@ -561,6 +504,67 @@ __device__ __forceinline__ void epilogue_frag_tma(const EpiArgs& p, const CUtens
     if (!full_c && nbase >= p.Cout) break;
     epilogue_frag_chunk<F, BN>(p, tmY, acc, cc, nbase, c1, c2, c3, pix, rpix, valid, alpha, stage, nbuf, sbuf, bar, leader);
   }
+}
+
+// ---------------------------------------------------------------------------------------- softmax rows in the fragment layout
+// A row's columns of the tile are held by the four lanes of a quad (lane q: columns 8j + 2q + 0 / 1), so every row reduction
+// is a reduction over this thread's columns and two xor shuffles (1, 2) within the quad; the results are the same in all four
+// lanes.  Every thread of the warp executes the shuffles, whatever its rows' validity.
+
+// Statistics pass (sm_mode 1) of one 64-row accumulator block: per row, (max, sum exp(. - max)) of the nchunk valid 64-column
+// chunks of the tile (channel tile `part`), stored by lane 0 of the quad; rows outside the output store nothing.
+template <int BN>
+__device__ __forceinline__ void epilogue_frag_smstats(const EpiArgs& p, const float (&acc)[BN / 2], int nchunk, int part,
+                                                      const long long (&pix)[2], const bool (&valid)[2], float alpha) {
+  const float a2 = alpha * kLog2e;
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    float m0 = -INFINITY, m1 = -INFINITY;       // two chains: one warp per scheduler runs this, so latency is not hidden
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+      if (j < 8 * nchunk) { m0 = fmaxf(m0, acc[4 * j + 2 * hr] * alpha); m1 = fmaxf(m1, acc[4 * j + 2 * hr + 1] * alpha); }
+    float m = fmaxf(m0, m1);
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+    const float m2 = -m * kLog2e;
+    float l0 = 0.f, l1 = 0.f;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+      if (j < 8 * nchunk) { l0 += fast_ex2(fmaf(acc[4 * j + 2 * hr], a2, m2)); l1 += fast_ex2(fmaf(acc[4 * j + 2 * hr + 1], a2, m2)); }
+    float l = l0 + l1;
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    if ((threadIdx.x & 3) == 0 && valid[hr]) reinterpret_cast<float2*>(p.sm_stats)[pix[hr] * p.sm_parts + part] = make_float2(m, l);
+  }
+}
+
+// Apply pass (sm_mode 2), first half: lane q of the quad merges the row's partials q, q + 4, q + 8, ...; this loads the first
+// two of them ((-inf, 0) past sm_parts and for rows outside the output).  Issued before the main loop, whose MMAs hide the load.
+__device__ __forceinline__ void sm_row_load(const EpiArgs& p, long long pix, bool valid, float2 (&t)[2]) {
+  const int q = threadIdx.x & 3;
+  const float2* st = reinterpret_cast<const float2*>(p.sm_stats) + pix * p.sm_parts;
+#pragma unroll
+  for (int k = 0; k < 2; ++k) t[k] = (valid && q + 4 * k < p.sm_parts) ? __ldcg(st + q + 4 * k) : make_float2(-INFINITY, 0.f);
+}
+
+// Apply pass, second half: merges t with this lane's further partials (sm_parts > 8) and across the quad into epi_pair's row
+// constants (-m log2e, 1 / l); (0, 1) for rows outside the output.
+__device__ __forceinline__ float2 sm_row_apply(const EpiArgs& p, long long pix, bool valid, const float2 (&t)[2]) {
+  const int q = threadIdx.x & 3;
+  const float2* st = reinterpret_cast<const float2*>(p.sm_stats) + pix * p.sm_parts;
+  float m = fmaxf(t[0].x, t[1].x);
+  for (int i = q + 8; valid && i < p.sm_parts; i += 4) m = fmaxf(m, __ldcg(&st[i].x));
+  m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+  m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+  // an absent partial (-inf, 0) adds 0 * ex2(-inf) = 0
+  float l = t[0].y * fast_ex2((t[0].x - m) * kLog2e) + t[1].y * fast_ex2((t[1].x - m) * kLog2e);
+  for (int i = q + 8; valid && i < p.sm_parts; i += 4) {
+    const float2 u = __ldcg(st + i);
+    l += u.y * fast_ex2((u.x - m) * kLog2e);
+  }
+  l += __shfl_xor_sync(0xffffffffu, l, 1);
+  l += __shfl_xor_sync(0xffffffffu, l, 2);
+  return valid ? make_float2(-m * kLog2e, 1.f / l) : make_float2(0.f, 1.f);
 }
 
 }  // namespace sgb

@@ -9,13 +9,14 @@
 //
 // One persistent CTA per SM, 3 warpgroups: warp 0 = TMA producer (one lane), warp 2 = auxiliary-operand producer (fprop),
 // warpgroups 1 and 2 = consumers.  The producer warpgroup drops to 40 registers (setmaxnreg), the consumers rise to 232.
-// fprop, compile-time epilogue variants (all but the softmax ones): ping-pong.  Each consumer warpgroup owns whole tiles
-// (local tile i -> warpgroup i & 1), issues two m64 wgmmas per K step (rows 0..63 / 64..127, 128 accumulator registers at
-// BN = 128) and, once its main loop is done, hands the tensor cores to the other warpgroup (named barriers) and runs the fused
-// epilogue straight from its registers: per 64-channel chunk and 64-row half, bf16 pairs into its own staging tiles and one TMA
-// store; residual / mask boxes arrive through its own aux ring.  The operand ring stays one ring in tile order.
-// fprop, run-time flags and softmax variants: both warpgroups run every tile (64 rows each), stage the accumulator tile in
-// shared memory as fp32 rows and run the epilogue on it (one thread = one row).
+// fprop, compile-time epilogue variants: ping-pong.  Each consumer warpgroup owns whole tiles (local tile i -> warpgroup
+// i & 1), issues two m64 wgmmas per K step (rows 0..63 / 64..127, 128 accumulator registers at BN = 128) and, once its main
+// loop is done, hands the tensor cores to the other warpgroup (named barriers) and runs the fused epilogue straight from its
+// registers: per 64-channel chunk and 64-row half, bf16 pairs into its own staging tiles and one TMA store; residual / mask /
+// softmax-P boxes arrive through its own aux ring; the attention softmax's row reductions run within the lane quads of the
+// accumulator fragment.  The operand ring stays one ring in tile order.
+// fprop, run-time flags (F = -1): both warpgroups run every tile (64 rows each), stage the accumulator tile in shared memory as
+// fp32 rows and run the epilogue on it (one thread = one row).
 // wgrad: each consumer warpgroup owns 64 of the tile's 128 rows; fp32 red.adds straight from the accumulator registers.
 #include "common.cuh"
 #include "ptx.cuh"
@@ -43,7 +44,7 @@ struct FpropArgs {
   int use_tma;                    // epilogue through staging tiles + TMA tensor stores
   int epi_nbuf;                   // staging tiles per epilogue team (2: stores overlap the next chunk's conversion)
   int b_resident;                 // 1: every weight tile of this CTA's channel tile stays in shared memory (loaded once)
-  int aux_kind, aux_tw, aux_th;   // residual (1) / mask (2) tile staged by TMA; its box is aux_tw x aux_th x nb pixels
+  int aux_kind, aux_tw, aux_th;   // residual (1) / mask (2) / softmax P (3) tile staged by TMA; box aux_tw x aux_th x nb pixels
   int aux_depth;                  // aux tiles per epilogue team (ring filled by the aux producer warp)
   int out_sub;                    // 2: store only even (h, w) outputs at (h/2, w/2) -> stride-2 convolution (Inception reduction blocks)
   EpiArgs e;
@@ -60,7 +61,7 @@ __device__ __forceinline__ FpropTile fprop_tile(const FpropArgs& p, int t) {
   return c;
 }
 
-__host__ __device__ constexpr bool fprop_is_pingpong(int f) { return f >= 0 && (f & (kEpiSmStats | kEpiSmApply | kEpiSmBwd)) == 0; }
+__host__ __device__ constexpr bool fprop_is_pingpong(int f) { return f >= 0; }
 
 // Shared memory of conv_fprop_kernel: addresses from base, or offsets from the 1024-aligned base when base = 0.  Every tile
 // region is a multiple of 1024 bytes (b_bytes too: BN % 8 == 0).
@@ -146,17 +147,18 @@ __device__ __forceinline__ void fprop_staged_mma(const FpropArgs& p, const Fprop
 }
 
 // ------------------------------------------------------------------------------------------------ fprop, ping-pong schedule
-// Compile-time epilogue variants other than the softmax ones: each consumer warpgroup owns whole 128-row tiles (local tile i
-// goes to warpgroup i & 1) and runs the epilogue straight from its registers while the other warpgroup issues its MMAs.
+// Compile-time epilogue variants: each consumer warpgroup owns whole 128-row tiles (local tile i goes to warpgroup i & 1) and
+// runs the epilogue straight from its registers while the other warpgroup issues its MMAs.
 static constexpr uint32_t kTurnBar = 4;       // named barriers 4 / 5: warpgroup 0 / 1 may start its next mainloop
 
 // One consumer warpgroup of the ping-pong schedule.  The two warpgroups' main loops take turns (named barriers kTurnBar + wg),
 // so warpgroup A's epilogue runs under warpgroup B's MMAs.  The epilogue stores the tile as two 64-row half boxes per
-// 64-channel chunk through this warpgroup's staging tiles; a residual / mask chunk arrives in this warpgroup's aux ring as one
-// box of the whole tile, read by both halves.
+// 64-channel chunk through this warpgroup's staging tiles; a residual / mask / softmax-P chunk arrives in this warpgroup's aux
+// ring as one box of the whole tile, read by both halves.  The softmax statistics pass stores only its row partials.
 template <int F, int BN>
 __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUtensorMap* tmY, const FpropSmem& L, int wg) {
-  constexpr int aux_kind = (F & kEpiAuxRes) ? 1 : ((F & kEpiAuxMask) ? 2 : 0);
+  constexpr int aux_kind = (F & kEpiAuxRes) ? 1 : ((F & kEpiAuxMask) ? 2 : ((F & kEpiSmBwd) ? 3 : 0));
+  constexpr bool sm_stats = (F & kEpiSmStats) != 0, sm_apply = (F & kEpiSmApply) != 0, sm_bwd = (F & kEpiSmBwd) != 0;
   const uint32_t w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const bool leader = (threadIdx.x & 127) == 0;
   const float alpha = epi_alpha(p.e);
@@ -185,10 +187,6 @@ __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUte
   for (int i = wg; i < n_local; i += 2) {
     const FpropTile tc = fprop_tile(p, (int)blockIdx.x + i * (int)gridDim.x);
     const int nt = tc.nt, wt = tc.wt, ht = tc.ht, bt = tc.bt;
-    float acc[2][BN / 2];
-    if (i > 0) named_bar_sync(kTurnBar + wg, 256);          // the other warpgroup has issued tile i - 1
-    fprop_mma<BN, 2>(p, L, acc, 0u, (uint32_t)(i * kiters));
-    if (i + 1 < n_local) named_bar_arrive(kTurnBar + (wg ^ 1), 256);
     long long pix[2][2], rpix[2][2];
     bool valid[2][2];
     int c1[2], c2[2], c3[2];
@@ -205,6 +203,32 @@ __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUte
         rpix[h][hr] = epi_rpix(p.e, b, y, x, p.H, p.W, pix[h][hr]);
       }
     }
+    // softmax row operands of this thread's four rows, loaded before the turn barrier: the other warpgroup's MMAs and this
+    // one's hide their latency.  sm: epi_pair's row constants (apply: merged after the main loop from the partials smt).
+    float2 sm[2][2] = {}, smt[2][2][2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        if (sm_apply) sm_row_load(p.e, pix[h][hr], valid[h][hr], smt[h][hr]);
+        if (sm_bwd) sm[h][hr].x = valid[h][hr] ? __ldg(p.e.sm_delta + pix[h][hr]) : 0.f;
+      }
+    float acc[2][BN / 2];
+    if (i > 0) named_bar_sync(kTurnBar + wg, 256);          // the other warpgroup has issued tile i - 1
+    fprop_mma<BN, 2>(p, L, acc, 0u, (uint32_t)(i * kiters));
+    if (i + 1 < n_local) named_bar_arrive(kTurnBar + (wg ^ 1), 256);
+    if constexpr (sm_stats) {
+      const int nchunk = min(BN, p.e.Cout - nt * BN) / 64;   // (a chunk past Cout holds the zero-filled B rows)
+      epilogue_frag_smstats<BN>(p.e, acc[0], nchunk, nt, pix[0], valid[0], alpha);
+      epilogue_frag_smstats<BN>(p.e, acc[1], nchunk, nt, pix[1], valid[1], alpha);
+      continue;
+    }
+    if (sm_apply) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) sm[h][hr] = sm_row_apply(p.e, pix[h][hr], valid[h][hr], smt[h][hr]);
+    }
 #pragma unroll                                    // static accumulator indices: the fragments stay in registers
     for (int cc = 0; cc * 64 < BN; ++cc) {
       const int nbase = nt * BN + cc * 64;
@@ -216,9 +240,9 @@ __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUte
         ++aux_cnt;
       }
       epilogue_frag_chunk<F, BN>(p.e, tmY, acc[0], cc, nbase, c1[0], c2[0], c3[0], pix[0], rpix[0], valid[0], alpha, stage,
-                                 p.epi_nbuf, sbuf, 1u + wg, leader, aux_tile, arow[0]);
+                                 p.epi_nbuf, sbuf, 1u + wg, leader, aux_tile, arow[0], sm[0]);
       epilogue_frag_chunk<F, BN>(p.e, tmY, acc[1], cc, nbase, c1[1], c2[1], c3[1], pix[1], rpix[1], valid[1], alpha, stage,
-                                 p.epi_nbuf, sbuf, 1u + wg, leader, aux_tile, arow[1]);
+                                 p.epi_nbuf, sbuf, 1u + wg, leader, aux_tile, arow[1], sm[1]);
       // every thread of the warpgroup is past its last read of the aux box (the barrier before the second half's store)
       if (aux_kind != 0 && leader) mbar_arrive(aux.empty(aslot));
     }
@@ -226,9 +250,8 @@ __device__ __forceinline__ void fprop_pp_consumer(const FpropArgs& p, const CUte
   if (leader) bulk_wait_all();                    // staging tiles must outlive the last tensor store
 }
 
-// Staged-epilogue consumer (run-time flags and softmax variants): both warpgroups run the MMAs of every tile, stage the
+// Staged-epilogue consumer (the run-time general kernel, F = -1): both warpgroups run the MMAs of every tile, stage the
 // accumulators in shared memory as fp32 rows, then run the epilogue on them.
-template <int F>
 __device__ __forceinline__ void fprop_staged_consumer(const FpropArgs& p, const CUtensorMap* tmY, const FpropSmem& L, int wg) {
   // Epilogue: team = which 64-channel chunks (even / odd) = consumer warpgroup, q = which 32 rows.
   const int ct = threadIdx.x - 128;
@@ -266,11 +289,9 @@ __device__ __forceinline__ void fprop_staged_consumer(const FpropArgs& p, const 
       case 64: fprop_staged_mma<64>(p, L, it, wg); break;
       default: fprop_staged_mma<128>(p, L, it, wg); break;
     }
-    if constexpr (F >= 0 && (F & kEpiSmStats) != 0) {
-      epilogue_tile_smstats(p.e, t_row, p.BN, n0, valid, pix, alpha, team, nt * 2 + team);
-    } else if (p.use_tma) {
-      epilogue_tile_tma<F>(p.e, tmY, t_row, p.BN, n0, wt * p.tw, ht * p.th, bt * p.nb, valid, pix, rpix, alpha, stage, p.epi_nbuf,
-                           sbuf, team, row, leader, p.aux_kind ? &aux : nullptr);
+    if (p.use_tma) {
+      epilogue_tile_tma(p.e, tmY, t_row, p.BN, n0, wt * p.tw, ht * p.th, bt * p.nb, valid, pix, rpix, alpha, stage, p.epi_nbuf,
+                        sbuf, team, row, leader, p.aux_kind ? &aux : nullptr);
     } else if (team == 0) {
       epilogue_row(p.e, t_row, p.BN, n0, valid, pix, rpix, alpha, vec_ok);
     }
@@ -308,7 +329,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (p.BN == 64) fprop_pp_consumer<F, 64>(p, &tmY, L, wg);
       else fprop_pp_consumer<F, 128>(p, &tmY, L, wg);
     } else {
-      fprop_staged_consumer<F>(p, &tmY, L, wg);
+      fprop_staged_consumer(p, &tmY, L, wg);
     }
     return;
   }
@@ -347,7 +368,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
   } else if (warp == 2) {
     if (lane == 0 && p.aux_kind) {
-      // ------------------------------------------------------------- aux producer: residual / mask boxes, in the order the
+      // ------------------------------------------------------------- aux producer: residual / mask / P boxes, in the order the
       // two rings are consumed (staged epilogue: team = chunk & 1; ping-pong: ring = local tile & 1), up to aux_depth boxes
       // ahead per ring
       const bool half = p.aux_kind == 1 && p.e.res_up2;
@@ -599,7 +620,7 @@ using namespace sgb;
 extern "C" int sgb_conv_softmax_parts(const sgb_conv_desc* d) {
   if (!d || d->Cout <= 0) return 0;
   const int BN = pick_bn(d);
-  return 2 * ((d->Cout + BN - 1) / BN);
+  return (d->Cout + BN - 1) / BN;       // one (max, sum exp) partial per row and channel tile
 }
 
 extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
@@ -656,18 +677,18 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
     else if (p.tw >= 2) { p.aux_kind = 1; p.aux_tw = p.tw / 2; p.aux_th = p.th >= 2 ? p.th / 2 : 1; }
   }
   if (d->sm_mode) {
-    SGB_REQUIRE(p.use_tma);                                            // (the softmax variants exist only for the staged-store epilogue)
+    SGB_REQUIRE(p.use_tma);                                            // (the softmax variants exist only for the TMA-store epilogue)
     if (d->sm_mode == 3) p.aux_kind = 3;                               // P tile of the softmax backward
   }
   fill_epi(p.e, d);
-  p.e.sm_parts = 2 * p.tiles_n;
+  p.e.sm_parts = p.tiles_n;
   int f = p.use_tma ? epi_flags_of(p.e) : -1;
   SGB_REQUIRE(!d->sm_mode || f == (kEpiFull | (d->sm_mode == 1 ? kEpiSmStats : d->sm_mode == 2 ? kEpiSmApply : kEpiSmBwd)));
   if (f >= 0 && p.aux_kind == 1) f |= kEpiAuxRes;
   if (f >= 0 && p.aux_kind == 2) f |= kEpiAuxMask;
   if (!FpropCompiled::has(f)) f = -1;
-  // ping-pong variants: no fp32 accumulator staging; 8 KiB half-tile staging tiles per warpgroup.  Staged variants: fp32 rows
-  // of the whole tile plus 16 KiB staging tiles per epilogue team.
+  // ping-pong (every compiled variant): no fp32 accumulator staging; 8 KiB half-tile staging tiles per warpgroup.  The general
+  // kernel (F = -1): fp32 rows of the whole tile plus 16 KiB staging tiles per epilogue team.
   const bool pingpong = fprop_is_pingpong(f);
   // short-K layers (one or two K blocks per tile) are store bound: their (small) filter stays resident in shared memory and the
   // space of the B halves of the ring buys more staging tiles per epilogue team = more store bytes in flight
@@ -675,6 +696,9 @@ extern "C" int sgb_conv_fprop(const sgb_conv_desc* d, sgb_stream_t stream_) {
   const int kt = p.taps * p.kblocks;
   p.b_resident = (d->w_mode == 0 && p.tiles_n == 1 && kt <= 2 && kt * b_tile <= 64u * 1024u) ? 1 : 0;
   p.epi_nbuf = !p.use_tma ? 1 : pingpong ? (kt <= 2 ? 4 : 2) : (kt <= 2 ? 2 : 1);
+  // softmax backward (K = c/2 = 256, P through a 2-deep aux ring of 16 KiB boxes): one staging tile per warpgroup leaves room for
+  // a 4th operand stage, measured 11 % faster at the flagship attention than 2 staging tiles and 3 stages
+  if (d->sm_mode == 3) p.epi_nbuf = 1;
   p.aux_depth = p.aux_kind ? 2 : 1;
   p.stages = 0;
   // room for the operand ring: 216 KiB less the layout in front of it
