@@ -287,6 +287,9 @@ int sgb_adam_ema_step(float* p, const float* g, float* m, float* v, int64_t n, f
 /* step_dev (optional): int32 step counter in device memory used for the bias corrections instead of `step`, so that a
  * captured CUDA graph of the update stays correct when replayed. */
 int sgb_ema_lerp(float* ema, const float* p, int64_t n, float decay, sgb_stream_t stream);
+/* WGAN weight clipping (replaces src/worker.py:490-492, p.data.clamp_(-c, c) per discriminator parameter): x clamped to
+ * [-c, c] in place over a flat fp32 arena, NaN propagated as torch.clamp does; c >= 0 (the arena's zero padding stays 0). */
+int sgb_clamp(float* x, int64_t n, float c, sgb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Gradient penalty (replaces utils/losses.py:268-275 cal_deriv + :301-316 cal_grad_penalty).
@@ -301,6 +304,19 @@ int sgb_gp_interpolate(const float* real, const float* fake, const float* alpha,
                        sgb_stream_t stream);
 int sgb_gp_sumsq(const float* g, float* sumsq, int32_t B, int64_t n_per, sgb_stream_t stream);
 int sgb_gp_seed(const float* g, const float* sumsq, float* v, int32_t B, int64_t n_per, sgb_stream_t stream);
+/* Max-gradient penalty (replaces utils/losses.py:337-353 cal_maxgrad_penalty): *penalty = P = max_b sumsq[b] and the seed
+ * v = dP/dg = 2 g_b / n_ties on the samples whose sumsq equals the maximum, 0 elsewhere (torch's backward of a full max()
+ * reduction splits the gradient evenly over ties).  sumsq: the per-sample output of sgb_gp_sumsq. */
+int sgb_gp_seed_max(const float* g, const float* sumsq, float* v, float* penalty, int32_t B, int64_t n_per, sgb_stream_t stream);
+/* DRAGAN perturbation (replaces utils/losses.py:319-335 cal_dra_penalty up to the discriminator call):
+ * sgb_dra_std: *sigma = real_images.std() (unbiased, over all n elements; fp64 accumulation, one fp32 result on the
+ *   device).  ws: fp64 scratch of 2 * SGB_DRA_STD_PARTS elements.
+ * sgb_dra_perturb: out = real + alpha[b] * ((0.5 * *sigma) * noise), rounded as torch evaluates that expression; alpha [B]
+ *   and noise (shaped like real) are the reference's host draws. */
+#define SGB_DRA_STD_PARTS 256
+int sgb_dra_std(const float* x, int64_t n, double* ws, float* sigma, sgb_stream_t stream);
+int sgb_dra_perturb(const float* real, const float* sigma, const float* alpha, const float* noise, float* out, int32_t B,
+                    int64_t n_per, sgb_stream_t stream);
 int sgb_bn_tangent_bwd_reduce(const void* x, int64_t x_cstride, const void* a, int64_t a_cstride, const void* c, int64_t c_cstride,
                               int64_t npix, int32_t C, const float* mean, const float* rstd, float* sums, sgb_stream_t stream);
 int sgb_bn_tangent_bwd_apply(const void* x, int64_t x_cstride, const void* a, int64_t a_cstride, const void* c, int64_t c_cstride,

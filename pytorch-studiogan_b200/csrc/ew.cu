@@ -721,6 +721,122 @@ __global__ void __launch_bounds__(256) gp_seed_kernel(const float* __restrict__ 
   }
 }
 
+// losses.cal_dra_penalty (src/utils/losses.py:319-335): sigma = real_images.std() (unbiased, over the whole batch) and
+// x_hat = real + alpha_b * ((0.5 * sigma) * u), each product and the sum rounded once, in torch's order.  The standard
+// deviation accumulates in fp64 around the first element (shifted sums keep the one-pass variance free of cancellation);
+// one block per slice writes its two partial sums, then a single block adds them in a fixed order: deterministic.
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ void block_sum2_f64(double& s, double& q) {    // 256 threads; the result lands in thread 0
+  __shared__ double red[2][8];
+  s = warp_sum_f64(s);
+  q = warp_sum_f64(q);
+  if ((threadIdx.x & 31) == 0) {
+    red[0][threadIdx.x >> 5] = s;
+    red[1][threadIdx.x >> 5] = q;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    s = q = 0.0;
+    for (int w = 0; w < 8; ++w) {
+      s += red[0][w];
+      q += red[1][w];
+    }
+  }
+}
+__global__ void __launch_bounds__(256) dra_std_partial_kernel(const float* __restrict__ x, long long n, double* __restrict__ ws) {
+  const double x0 = (double)__ldg(x);
+  double s = 0.0, q = 0.0;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+    const double d = (double)__ldg(x + i) - x0;
+    s += d;
+    q = fma(d, d, q);
+  }
+  block_sum2_f64(s, q);
+  if (threadIdx.x == 0) {
+    ws[2 * blockIdx.x] = s;
+    ws[2 * blockIdx.x + 1] = q;
+  }
+}
+__global__ void __launch_bounds__(256) dra_std_final_kernel(const double* __restrict__ ws, int parts, long long n,
+                                                             float* __restrict__ sigma) {
+  double s = 0.0, q = 0.0;
+  for (int k = threadIdx.x; k < parts; k += 256) {
+    s += ws[2 * k];
+    q += ws[2 * k + 1];
+  }
+  block_sum2_f64(s, q);
+  if (threadIdx.x == 0) {
+    const double var = fmax((q - s * s / (double)n) / (double)(n - 1), 0.0);
+    *sigma = (float)sqrt(var);
+  }
+}
+__global__ void __launch_bounds__(256) dra_perturb_kernel(const float* __restrict__ real, const float* __restrict__ sigma,
+                                                           const float* __restrict__ alpha, const float* __restrict__ noise,
+                                                           float* __restrict__ out, long long n_per, long long total) {
+  const float half_sigma = __fmul_rn(0.5f, __ldg(sigma));
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const float a = __ldg(alpha + i / n_per);
+    out[i] = __fadd_rn(real[i], __fmul_rn(a, __fmul_rn(half_sigma, noise[i])));
+  }
+}
+
+// losses.cal_maxgrad_penalty (src/utils/losses.py:337-353): P = max_b ||g_b||^2 and its gradient w.r.t. g, which torch's
+// backward of a full max() reduction spreads evenly over the tied arg-max samples: v_b = 2 g_b / n_ties there, 0
+// elsewhere.  A NaN norm makes P NaN and the NaN samples the arg-max, as torch's max does.  Every block finds the maximum
+// and the tie count over the [B] norms itself (B is small) before its slice of v.
+__global__ void __launch_bounds__(256) gp_seed_max_kernel(const float* __restrict__ g, const float* __restrict__ sumsq,
+                                                           float* __restrict__ v, float* __restrict__ penalty, int B,
+                                                           long long n_per, long long total) {
+  __shared__ float red[8];
+  __shared__ float s_max;
+  __shared__ int s_ties;
+  float m = -INFINITY;
+  int nan = 0;
+  for (int b = threadIdx.x; b < B; b += 256) {
+    const float s = __ldg(sumsq + b);
+    nan |= isnan(s);
+    m = fmaxf(m, s);
+  }
+  nan = __syncthreads_or(nan);
+  m = warp_max(m);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = red[0];
+    for (int w = 1; w < 8; ++w) t = fmaxf(t, red[w]);
+    s_max = nan ? __int_as_float(0x7fffffff) : t;
+    s_ties = 0;
+  }
+  __syncthreads();
+  m = s_max;
+  int ties = 0;
+  for (int b = threadIdx.x; b < B; b += 256) {
+    const float s = __ldg(sumsq + b);
+    ties += nan ? isnan(s) : s == m;
+  }
+  if (ties) atomicAdd(&s_ties, ties);
+  __syncthreads();
+  if (blockIdx.x == 0 && threadIdx.x == 0) *penalty = m;
+  const float coef = 2.f / (float)s_ties;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const float s = __ldg(sumsq + i / n_per);
+    v[i] = (nan ? isnan(s) : s == m) ? coef * g[i] : 0.f;
+  }
+}
+
+// WGAN weight clipping (src/worker.py:490-492, p.data.clamp_(-c, c) over every discriminator parameter) as torch.clamp:
+// NaN stays NaN, which fminf / fmaxf alone would replace by a bound.
+__global__ void __launch_bounds__(256) clamp_kernel(float* __restrict__ x, long long n, float c) {
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+    const float t = x[i];
+    x[i] = isnan(t) ? t : fminf(fmaxf(t, -c), c);
+  }
+}
+
 }  // namespace sgb
 
 using namespace sgb;
@@ -1007,6 +1123,46 @@ extern "C" int sgb_gp_seed(const float* g, const float* sumsq, float* v, int32_t
   SGB_REQUIRE(g && sumsq && v && B > 0 && n_per > 0);
   const long long total = (long long)B * n_per;
   gp_seed_kernel<<<ew_blocks(total), 256, 0, stream>>>(g, sumsq, v, n_per, total, 1.f / (float)B);
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
+extern "C" int sgb_gp_seed_max(const float* g, const float* sumsq, float* v, float* penalty, int32_t B, int64_t n_per,
+                               sgb_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  SGB_REQUIRE(g && sumsq && v && penalty && B > 0 && n_per > 0);
+  const long long total = (long long)B * n_per;
+  gp_seed_max_kernel<<<ew_blocks(total), 256, 0, stream>>>(g, sumsq, v, penalty, B, n_per, total);
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
+extern "C" int sgb_dra_std(const float* x, int64_t n, double* ws, float* sigma, sgb_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  SGB_REQUIRE(x && ws && sigma && n > 1);
+  long long parts = (n + 256 * 16 - 1) / (256 * 16);
+  if (parts > SGB_DRA_STD_PARTS) parts = SGB_DRA_STD_PARTS;
+  dra_std_partial_kernel<<<(unsigned)parts, 256, 0, stream>>>(x, n, ws);
+  SGB_LAUNCH_CHECK();
+  dra_std_final_kernel<<<1, 256, 0, stream>>>(ws, (int)parts, n, sigma);
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
+extern "C" int sgb_dra_perturb(const float* real, const float* sigma, const float* alpha, const float* noise, float* out,
+                               int32_t B, int64_t n_per, sgb_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  SGB_REQUIRE(real && sigma && alpha && noise && out && B > 0 && n_per > 0);
+  const long long total = (long long)B * n_per;
+  dra_perturb_kernel<<<ew_blocks(total), 256, 0, stream>>>(real, sigma, alpha, noise, out, n_per, total);
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
+extern "C" int sgb_clamp(float* x, int64_t n, float c, sgb_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  SGB_REQUIRE(x && n > 0 && c >= 0.f);
+  clamp_kernel<<<ew_blocks(n), 256, 0, stream>>>(x, n, c);
   SGB_LAUNCH_CHECK();
   return SGB_OK;
 }

@@ -107,6 +107,10 @@ SIGNATURES = {
     "sgb_gp_interpolate": (c_int, [c_p, c_p, c_p, c_p, c_int, c_i64, c_p]),
     "sgb_gp_sumsq": (c_int, [c_p, c_p, c_int, c_i64, c_p]),
     "sgb_gp_seed": (c_int, [c_p, c_p, c_p, c_int, c_i64, c_p]),
+    "sgb_gp_seed_max": (c_int, [c_p, c_p, c_p, c_p, c_int, c_i64, c_p]),
+    "sgb_dra_std": (c_int, [c_p, c_i64, c_p, c_p, c_p]),
+    "sgb_dra_perturb": (c_int, [c_p, c_p, c_p, c_p, c_p, c_int, c_i64, c_p]),
+    "sgb_clamp": (c_int, [c_p, c_i64, c_f, c_p]),
     "sgb_sample_mean": (c_int, [c_p, c_int, c_i64, c_p, c_p]),
     "sgb_diffaug_fwd": (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_p]),
     "sgb_diffaug_bwd": (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_p]),

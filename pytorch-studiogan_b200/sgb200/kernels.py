@@ -522,6 +522,43 @@ def gp_seed(g, sumsq):
     return v
 
 
+def gp_seed_max(g, sumsq):
+    """(P = max_b sumsq[b] as a 0-dim device tensor, v = dP/dg with ties split evenly)."""
+    g = g.contiguous()
+    B = g.shape[0]
+    v = torch.empty_like(g)
+    penalty = torch.empty((), device=g.device, dtype=torch.float32)
+    L.call("sgb_gp_seed_max", L.ptr(g), L.ptr(sumsq), L.ptr(v), L.ptr(penalty), B, g.numel() // B, _s())
+    return penalty, v
+
+
+DRA_STD_PARTS = 256                                   # SGB_DRA_STD_PARTS (include/sgb200.h)
+
+
+def dra_std(x):
+    """Unbiased standard deviation of all elements of a contiguous fp32 tensor, as a [1] device tensor."""
+    x = x.contiguous()
+    ws = torch.empty(2 * DRA_STD_PARTS, device=x.device, dtype=torch.float64)
+    sigma = torch.empty(1, device=x.device, dtype=torch.float32)
+    L.call("sgb_dra_std", L.ptr(x), x.numel(), L.ptr(ws), L.ptr(sigma), _s())
+    return sigma
+
+
+def dra_perturb(real, sigma, alpha, noise):
+    """real + alpha[b] * ((0.5 * sigma) * noise) on contiguous fp32 [B, ...] tensors (torch's operation order)."""
+    real, noise = real.contiguous(), noise.contiguous()
+    out = torch.empty_like(real)
+    B = real.shape[0]
+    L.call("sgb_dra_perturb", L.ptr(real), L.ptr(sigma), L.ptr(alpha), L.ptr(noise), L.ptr(out), B, real.numel() // B, _s())
+    return out
+
+
+def clamp_(x, c):
+    """x.clamp_(-c, c) in place on a contiguous fp32 tensor (torch.clamp semantics: NaN stays NaN)."""
+    L.call("sgb_clamp", L.ptr(x), x.numel(), float(c), _s())
+    return x
+
+
 def bn_tangent_bwd_reduce(x, a, c, mean, rstd):
     B, C, H, W, xs = geom(x)
     sums = torch.empty((5, C), device=x.device, dtype=torch.float32)

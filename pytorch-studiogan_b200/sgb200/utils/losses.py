@@ -74,6 +74,18 @@ def cal_grad_penalty(real_images, real_labels, fake_images, discriminator, devic
     return gp.cal_grad_penalty(real_images, real_labels, fake_images, discriminator, device, alpha)
 
 
+def cal_dra_penalty(real_images, real_labels, discriminator, device=None, alpha=None, noise=None):
+    """src/utils/losses.py:319-335 (DRAGAN); see utils/gp.py."""
+    from . import gp
+    return gp.cal_dra_penalty(real_images, real_labels, discriminator, device, alpha, noise)
+
+
+def cal_maxgrad_penalty(real_images, real_labels, fake_images, discriminator, device=None, alpha=None):
+    """src/utils/losses.py:337-353 (LGAN max-gradient penalty); see utils/gp.py."""
+    from . import gp
+    return gp.cal_maxgrad_penalty(real_images, real_labels, fake_images, discriminator, device, alpha)
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # Class-conditioning losses of the classifier-based GANs (ACGAN "AC", ContraGAN "2C", ReACGAN "D2DCE"):
 # reference src/utils/losses.py:38-165.  They act on the discriminator head's [B, .] fp32 outputs; the label masks are

@@ -8,8 +8,10 @@ fp32 accumulation and fp32 master weights, which needs no loss scaling.
 import torch
 
 from . import _lib
+from . import kernels as K
 from .models import model as model_lib
 from .utils import losses, misc, sample
+from .utils.optim import ArenaAdam
 
 
 class _GraphedPhase:
@@ -96,7 +98,7 @@ class WORKER(object):
             self.cond_loss_mi = copy.deepcopy(self.cond_loss)
         if self.MODEL.aux_cls_type not in ("W/O", "N/A", "TAC", "ADC"):
             raise NotImplementedError("aux_cls_type %s" % self.MODEL.aux_cls_type)
-        for flag in ("apply_lo", "apply_topk", "apply_r1_reg", "apply_dra", "apply_maxgp", "apply_fm", "apply_wc", "apply_inv_reg"):
+        for flag in ("apply_lo", "apply_topk", "apply_r1_reg", "apply_fm", "apply_inv_reg"):
             if getattr(self.LOSS, flag, False):
                 raise NotImplementedError("LOSS.%s is outside the sgb200 hot-path scope" % flag)
         # a YAML that asks for an augmentation this path does not implement must not silently train a different recipe
@@ -144,7 +146,8 @@ class WORKER(object):
     def _graphs_enabled(self):
         plain = not (self.LOSS.apply_cr or self.LOSS.apply_bcr or self.LOSS.apply_zcr or self.LOSS.apply_lecam or
                      getattr(self.AUG, "apply_diffaug", False))      # host-side RNG / EMA state: not capturable
-        return bool(getattr(self.RUN, "cuda_graphs", False)) and not self.LOSS.apply_gp and self.cond_loss is None and plain
+        penalties = self.LOSS.apply_gp or self.LOSS.apply_dra or self.LOSS.apply_maxgp      # alpha / noise: host RNG draws
+        return bool(getattr(self.RUN, "cuda_graphs", False)) and not penalties and self.cond_loss is None and plain
 
     def train_discriminator(self, current_step):
         self._current_step = current_step
@@ -228,9 +231,16 @@ class WORKER(object):
                     if self._current_step > self.LOSS.lecam_ema_start_iter:
                         dis_acml_loss = dis_acml_loss + self.LOSS.lecam_lambda * losses.lecam_reg(
                             real_dict["adv_output"], fake_dict["adv_output"], self.lecam_ema)
+                # src/worker.py:369-392, in this order: each penalty draws its alpha (and DRAGAN its noise) from the host RNG
                 if self.LOSS.apply_gp:
-                    from .utils import gp
-                    dis_acml_loss = dis_acml_loss + self.LOSS.gp_lambda * gp.cal_grad_penalty(
+                    dis_acml_loss = dis_acml_loss + self.LOSS.gp_lambda * losses.cal_grad_penalty(
+                        real_images=real_images, real_labels=real_labels, fake_images=fake_images, discriminator=self.Dis,
+                        device=self.local_rank)
+                if self.LOSS.apply_dra:
+                    dis_acml_loss = dis_acml_loss + self.LOSS.dra_lambda * losses.cal_dra_penalty(
+                        real_images=real_images, real_labels=real_labels, discriminator=self.Dis, device=self.local_rank)
+                if self.LOSS.apply_maxgp:
+                    dis_acml_loss = dis_acml_loss + self.LOSS.maxgp_lambda * losses.cal_maxgrad_penalty(
                         real_images=real_images, real_labels=real_labels, fake_images=fake_images, discriminator=self.Dis,
                         device=self.local_rank)
                 dis_acml_loss = dis_acml_loss / self.OPTIMIZATION.acml_steps
@@ -238,7 +248,20 @@ class WORKER(object):
                 batch_counter += 1
             model_lib.allreduce_gradients(self.Dis, self.OPTIMIZATION.d_optimizer)
             self.OPTIMIZATION.d_optimizer.step()
+            if self.LOSS.apply_wc:
+                self._clip_discriminator_weights()
         return dis_acml_loss.detach()
+
+    @torch.no_grad()
+    def _clip_discriminator_weights(self):
+        """WGAN weight clipping after every discriminator update (src/worker.py:490-492): every D parameter into
+        [-wc_bound, wc_bound], frozen ones included.  With the arena optimiser that is one launch over the flat arena."""
+        c = float(self.LOSS.wc_bound)
+        if isinstance(self.OPTIMIZATION.d_optimizer, ArenaAdam):
+            K.clamp_(self.OPTIMIZATION.d_optimizer.arena.flat, c)
+        else:
+            for p in self.Dis.parameters():
+                p.data.clamp_(-c, c)
 
     # ------------------------------------------------------------------------------------------------ G phase
     def train_generator(self, current_step):
