@@ -57,6 +57,31 @@ def _s():
 
 
 # ---------------------------------------------------------------------------------------------- conv engine
+def _sm_count(device):
+    n = _SM_COUNT.get(device.index)
+    if n is None:
+        n = _SM_COUNT[device.index] = torch.cuda.get_device_properties(device).multi_processor_count
+    return n
+
+
+_SM_COUNT = {}
+
+
+def rows_segment(B, H, W, Cin, Cout, device):
+    """Segment width the halo-row kernel runs a stride-1 3x3 / pad 1 conv at (csrc/umma_conv3x3.cu rows_segment), 0 where the
+    generic kernel takes it: 128 when W % 128 == 0; 64 when W % 64 == 0 and its 256-pixel items (4 rows x 64 pixels x one
+    output-channel tile) number at least the SMs."""
+    if Cin % 64 != 0 or Cin > 256 or Cout % 8 != 0:
+        return 0
+    if W % 128 == 0 and H % 2 == 0:
+        return 128
+    if W % 64 == 0 and H % 4 == 0:
+        BN = 16 if Cout <= 16 else 32 if Cout <= 32 else 64 if Cout <= 64 else 128       # pick_bn of csrc/umma_conv.cu
+        if -(-Cout // BN) * (W // 64) * (H // 4) * B >= _sm_count(device):
+            return 64
+    return 0
+
+
 def conv_fprop(x, w, Cout, KH, KW, pad_h, pad_w, bias=None, residual=None, res_up2=False, res_after_mask=False,
                mask=None, relu=False, alpha=1.0, alpha_ptr=None, out=None, out_fp32=False, w_mode=0, same_size=True, stride=1,
                res_scale=1.0, mask_bits=None, want_relu_bits=False, sm_mode=0, sm_stats=None, sm_delta=None, sm_p=None):
@@ -126,8 +151,8 @@ def conv_fprop(x, w, Cout, KH, KW, pad_h, pad_w, bias=None, residual=None, res_u
         nb += 2.0 * B * H * W * Cout
     # accounting kind = the kernel the library dispatches (csrc/umma_conv3x3.cu conv3x3_rows_eligible): the halo-row kernel, the
     # generic kernel on a k x k filter (tensor bound) or on a 1x1 filter (HBM bound at these channel counts)
-    rows = (KH == 3 and KW == 3 and pad_h == 1 and pad_w == 1 and w_mode == 0 and same_size and stride == 1 and W % 128 == 0
-            and H % 2 == 0 and Cin % 64 == 0 and Cin <= 128 and Cout % 8 == 0)
+    rows = (KH == 3 and KW == 3 and pad_h == 1 and pad_w == 1 and w_mode == 0 and same_size and stride == 1
+            and rows_segment(B, H, W, Cin, Cout, x.device) != 0)
     kind = "conv3x3_rows" if rows else ("conv_fprop_1x1" if KH * KW == 1 else "conv_fprop_kxk")
     L.call("sgb_conv_fprop", ctypes.byref(d), _s(), tag="%s %dx%d %d->%d @%dx%d m%d" % (kind, KH, KW, Cin, Cout, H, W, w_mode),
            flops=2.0 * B * H * W * Cout * Cin * KH * KW, nbytes=nb)
